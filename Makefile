@@ -1,10 +1,10 @@
-# Builds the product library (CUDA, sm_100a) and the test oracle (CPU).
+# Builds the product library (CUDA, sm_90a) and the test oracle (CPU).
 #   make            -> xllm_service_b200/libxllm_ingest.so + oracle/liboracle.so
-#   make lib | oracle | ref | clean      (ref = oracle/_ref/libxllm_ref.so, the reference's own files; needs /root/reference)
+#   make lib | oracle | ref | clean      (ref = oracle/_ref/libxllm_ref.so, the reference's own files; needs the reference checkout, XLLM_REFERENCE_DIR)
 NVCC      ?= /usr/local/cuda/bin/nvcc
 CXX       ?= g++
 CC        ?= gcc
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVCCFLAGS := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC,-Wall,-Wno-unused-function -Iinclude --expt-relaxed-constexpr
 PKG       := xllm_service_b200
 CSRC      := $(PKG)/csrc

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """bench.py — requests/sec through tokenize + block-hash + prefix-match (+ cache-aware routing) at
-4K-token prompts (BASELINE.json metric) on N B200s, next to the CPU oracle on the host cores.
+4K-token prompts (BASELINE.json metric) on N H100s, next to the CPU oracle on the host cores.
 
   python bench.py --gpus N --steps K --warmup W          # this repo's CUDA path
   python bench.py --impl reference --gpus N ...          # the reference's CPU path (oracle port)
@@ -55,7 +55,55 @@ def parse_args():
     ap.add_argument("--index", default="auto", choices=["auto", "replicated", "sharded"],
                     help="prefix index placement at N > 1: sharded = BASELINE config 4 (hash-range shards, index N x "
                          "--index-keys, one NCCL all-to-all each way per batch); auto = sharded when N > 1")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the device-resident path returned in its last step (rank "
+                         "0) as DIR/<name>.npy in float64: per-request scalars, token ids, block keys and match "
+                         "scores, each over a fixed seeded sample of the requests (at most 64 MB in all)")
     return ap.parse_args()
+
+
+DUMP_SAMPLE_SEED = 12345
+DUMP_WIDE_BYTES = 44 << 20     # dump budget of the per-request rows (token ids, block keys, match scores)
+DUMP_SCALAR_BYTES = 16 << 20   # dump budget of the 11 per-request scalars
+
+
+def dump_outputs(out_dir, n, T, nb, d_ids, d_nids, d_st, d_keys, d_match, d_route):
+    """Writes the last timed step's outputs as float64 .npy files (every value is exact in float64: ids are int32,
+    the instance bitmask is split into two 32-bit halves, keys are written byte by byte).  Requests are sorted draws
+    of a fixed seed (wide_rows.npy, scalar_rows.npy; all requests when they fit), sized to keep the dump within
+    64 MB."""
+    import torch
+    from xllm_service_b200 import _lib
+    os.makedirs(out_dir, exist_ok=True)
+
+    def sample(k):
+        k = max(1, min(n, k))
+        return np.arange(n) if k == n else np.sort(np.random.default_rng(DUMP_SAMPLE_SEED).choice(n, k, replace=False))
+
+    wide = sample(DUMP_WIDE_BYTES // (8 * (T + nb * 16 + 3 * 64)))
+    scal = sample(DUMP_SCALAR_BYTES // (8 * 11))
+    sel = torch.from_numpy(wide).to(d_ids.device)
+    match = d_match.cpu().numpy().view(_lib.MATCH_DTYPE)[:, 0]
+    route = d_route.cpu().numpy().view(_lib.ROUTING_DTYPE)[:, 0]
+    arrays = {
+        "wide_rows": wide,
+        "ids": d_ids.index_select(0, sel).cpu().numpy(),
+        "keys": d_keys.index_select(0, sel).cpu().numpy().reshape(wide.size, nb * 16),
+        "match_hbm": match["hbm"][wide],
+        "match_dram": match["dram"][wide],
+        "match_ssd": match["ssd"][wide],
+        "scalar_rows": scal,
+        "n_ids": d_nids.cpu().numpy()[scal],
+        "status": d_st.cpu().numpy()[scal],
+        "match_max_block_num": match["max_block_num"][scal],
+        "match_max_matched_block_num": match["max_matched_block_num"][scal],
+        "match_instances_lo": match["instances"][scal] & 0xFFFFFFFF,
+        "match_instances_hi": match["instances"][scal] >> 32,
+    }
+    for f, _ in _lib.ROUTING_DTYPE:
+        arrays["route_" + f] = route[f][scal]
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
 
 
 def host_threads():
@@ -154,7 +202,7 @@ def instance_view(rng):
 
 # ----------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -204,16 +252,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def traffic_from_profiles(kernel):
-    """dram bytes per launch of `kernel` from the committed ncu capture of this command, or None."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            return json.load(f).get(kernel)
-    return None
+    return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s)"
 
 
 # ----------------------------------------------------------------------------------------------
@@ -791,6 +830,8 @@ def main():
     k_ms = np.array([[e[i].elapsed_time(e[i + 1]) for i in range(3)] for e in ev]).mean(axis=0)
     assert (torch.equal(d_ids.cpu(), torch.from_numpy(h_ids.numpy())) and
             torch.equal(d_keys.cpu(), torch.from_numpy(h_keys.numpy()))), "device-resident != e2e results"
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, n, T, nb, d_ids, d_nids, d_st, d_keys, d_match, d_route)
 
     shard_stats = h.shard_last_stats() if sharded_mode else None   # the last device-resident step's round
 
@@ -875,7 +916,7 @@ def main():
         k["frac"] = k["GBps"] / peak
     dom = max(kernels, key=lambda k: kernels[k]["ms"])
     roofline = {"kernel": dom, "bound": "hbm", "achieved": kernels[dom]["GBps"], "peak": peak, "unit": "GB/s",
-                "frac": kernels[dom]["frac"], "traffic": traffic_from_profiles(dom), "peak_source": peak_src,
+                "frac": kernels[dom]["frac"], "peak_source": peak_src,
                 "share_of_step": float(k_ms[list(kernels).index(dom)] / k_ms.sum()),
                 "note": "achieved = (text bytes + 4 B/token) / CUDA-event time of the encode launches (memo clear + "
                         "sp_express_kernel + the buffer-path and long-word kernels, empty grids on this workload); the "

@@ -1,7 +1,7 @@
 /*
- * xllm_ingest.h — C-ABI of the B200 request-ingest + prefix-cache routing path.
+ * xllm_ingest.h — C-ABI of the H100 request-ingest + prefix-cache routing path.
  *
- * One shared library, libxllm_ingest.so (CUDA, sm_100a), replaces the CPU hot path
+ * One shared library, libxllm_ingest.so (CUDA, sm_90a), replaces the CPU hot path
  * every request to an xllm-service front door traverses before PD dispatch:
  *
  *   Tokenizer::encode            xllm_service/tokenizer/tokenizer.h:32-33

@@ -4,7 +4,7 @@
 //   xllm_service/tokenizer/tokenizer_factory.cpp:14-19    tokenizer.json present -> FastTokenizer
 //   xllm_service/tokenizer/fast_tokenizer.cpp:20-30       encode = tokenizers_encode(text, add_special_tokens = 1); REPLACES *ids
 //   xllm_service/tokenizer/tokenizers/src/lib.rs:38-41,83-99   Tokenizer::encode(text, add_special_tokens)
-// The arithmetic is the Rust crate `tokenizers` 0.21 (Cargo.toml:11, absent from /root/reference); this file
+// The arithmetic is the Rust crate `tokenizers` 0.21 (Cargo.toml:11, absent from the reference checkout); this file
 // restates its published pipeline for the configuration GPT-2 style models use:
 //   added_vocabulary.rs   text is first split on the added (special) tokens, leftmost-longest
 //   pre_tokenizers/byte_level.rs   regex split

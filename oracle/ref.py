@@ -15,7 +15,7 @@ _lib = None
 
 
 def build():
-    """Compile oracle/_ref from /root/reference when that tree is present (no-op on the GPU box)."""
+    """Compile oracle/_ref from the reference checkout when that tree is present."""
     subprocess.check_call(["bash", os.path.join(_HERE, "build_ref.sh")])
 
 
@@ -32,7 +32,7 @@ def lib():
     global _lib
     if _lib is None:
         if not available():
-            raise RuntimeError("oracle/_ref/libxllm_ref.so is not built (needs /root/reference: bash oracle/build_ref.sh)")
+            raise RuntimeError("oracle/_ref/libxllm_ref.so is not built (needs the reference checkout: bash oracle/build_ref.sh)")
         L = ctypes.CDLL(_LIB_PATH)
         VP, I, SZ = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t
         L.ref_xxh3_128bits_hash.argtypes = [VP, VP, SZ, ctypes.c_uint32, VP]

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE — the C entry points of oracle/_ref/libxllm_ref.so.
 //
 // libxllm_ref.so is the REFERENCE ITSELF for rows a5-a8 / f1 / f3 of the hot path: oracle/build_ref.sh compiles
-// these reference files UNMODIFIED, where they lie under /root/reference/xllm_service, against the stand-in headers
+// these reference files UNMODIFIED, where they lie under the reference checkout's xllm_service/, against the stand-in headers
 // in oracle/ref_shim/stubs (glog, gflags, absl::Mutex, an in-memory etcd, hand-written protobuf accessors):
 //   common/hash_util.cpp            xxh3_128bits_hash                                   (a5)
 //   common/types.h                  CacheLocations JSON, OverlapScores, LoadBalanceInfos (a6, f3)

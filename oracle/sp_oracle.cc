@@ -11,7 +11,7 @@
 //
 // All arithmetic lives in the third-party library the reference links:
 //   sentencepiece @ ca10c9975797a4979b3c9fde33a14b2f92d1961d (third_party/sentencepiece, absent
-//   from /root/reference).  This file restates its published algorithm for BPE models:
+//   from the reference checkout).  This file restates its published algorithm for BPE models:
 //     normalizer.cc  Normalizer::Normalize / NormalizePrefix (precompiled charsmap = Darts
 //                    double-array trie + replacement blob; whitespace rules)
 //     bpe_model.cc   Model::Encode (agenda of adjacent symbol pairs: highest score first,

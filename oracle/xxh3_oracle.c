@@ -19,7 +19,7 @@
  *       zero-extended to XXH64_hash_t.
  *
  * Third-party arithmetic: xxHash (submodule third_party/xxHash @ ce037363, absent
- * from /root/reference).  XXH3 output is frozen since v0.8.0; this file restates
+ * from the reference checkout).  XXH3 output is frozen since v0.8.0; this file restates
  * the published algorithm (all four length classes + the long path with scramble)
  * and is pinned against libxxhash.so.0.8.2 and the vendored xxhash.h v0.8.3 by
  * tests/test_oracle_xxh3.py and the committed vectors in tests/golden/xxh3_kat.json.

@@ -15,6 +15,9 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import xllm_service_b200 as x  # noqa: E402
+from bench import peaks  # noqa: E402
+
+PEAK_GBPS, PEAK_SRC = peaks()
 from xllm_service_b200 import workload  # noqa: E402
 
 ap = argparse.ArgumentParser()
@@ -109,5 +112,5 @@ elif a.check:
 ms = sorted(ts)[len(ts) // 2]
 byts = batch.text.size + 4 * n_tok
 print(json.dumps({"kernel": "sp_encode", "backend": a.backend, "tokens_per_prompt": n_tok / a.n, **extra, "n": a.n, "T": a.T, "ms_median": ms, "ms_min": min(ts),
-                  "algo_GBps": byts / ms / 1e6, "frac_of_6585": byts / ms / 1e6 / 6585.1,
+                  "algo_GBps": byts / ms / 1e6, "frac_of_peak": byts / ms / 1e6 / PEAK_GBPS, "peak_source": PEAK_SRC,
                   "req_per_s": a.n / ms * 1e3, "text_bytes_per_prompt": batch.text.size / a.n}))

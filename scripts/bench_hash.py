@@ -10,6 +10,9 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import xllm_service_b200 as x  # noqa: E402
+from bench import peaks  # noqa: E402
+
+PEAK_GBPS, PEAK_SRC = peaks()
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--n", type=int, default=65536)
@@ -52,5 +55,5 @@ for _ in range(a.iters):
 ms = sorted(ts)[len(ts) // 2]
 byts = n * nb * 528
 print(json.dumps({"kernel": "xxh3_chain128", "n": n, "T": T, "ms_median": ms, "ms_min": min(ts),
-                  "GBps": byts / ms / 1e6, "frac_of_6585": byts / ms / 1e6 / 6585.1,
+                  "GBps": byts / ms / 1e6, "frac_of_peak": byts / ms / 1e6 / PEAK_GBPS, "peak_source": PEAK_SRC,
                   "req_per_s": n / ms * 1e3}))

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (select with -m gpu)")
     config.addinivalue_line("markers", "sweep: exhaustive device-vs-oracle Unicode sweeps (also marked gpu; -m sweep selects "
                                        "them alone)")
 

@@ -1,5 +1,5 @@
 // The drop-in boundary, proven by compiling the reference's own files against it (built by oracle/build_ref.sh into
-// oracle/_ref/reference_seams_test, because it needs /root/reference's headers; run on the GPU by
+// oracle/_ref/reference_seams_test, because it needs the reference checkout's headers; run on the GPU by
 // tests/test_gpu_reference_seams.py):
 //   fast  : the reference's tokenizer/fast_tokenizer.cpp, UNMODIFIED, linked against libxllm_ingest.so — its
 //           FastTokenizer class (fast_tokenizer.h) drives tokenizers_new_from_path / _encode / _decode /
@@ -100,7 +100,7 @@ static int run_route(uint64_t seed) {
   auto ref_mgr = std::make_shared<GlobalKVCacheMgr>(opt, etcd, true);
   auto ref_inst = std::make_shared<InstanceMgr>();
   CacheAwareRouting ref_car(ref_inst, ref_mgr);
-  // B200 side
+  // GPU side
   xllm_ingest_config cfg{};
   cfg.block_size = 128;
   cfg.xxh3_seed = 1024;

@@ -1,5 +1,5 @@
 """The drop-in boundary exercised through the reference's OWN code (oracle/_ref/reference_seams_test, built by
-oracle/build_ref.sh from tests/cpp/reference_seams_main.cc — it needs /root/reference's headers, so the binary is
+oracle/build_ref.sh from tests/cpp/reference_seams_main.cc — it needs the reference checkout's headers, so the binary is
 prebuilt in the build container and travels to the GPU box like the .so files):
   * the reference's tokenizer/fast_tokenizer.cpp, compiled UNMODIFIED and linked against libxllm_ingest.so, runs the
     pip-`tokenizers` goldens through FastTokenizer::encode / decode / token_to_id / id_to_token / vocab_size / clone;

@@ -1,9 +1,9 @@
 """Rows a5-a8 / f1 / f3 pinned to the REFERENCE ITSELF: oracle/_ref/libxllm_ref.so is the reference's own
 hash_util.cpp, types.h, global_kvcache_mgr.cpp, etcd_client.cpp, cache_aware_routing.cpp and
-InstanceMgr::get_load_metrics compiled unmodified from /root/reference (oracle/build_ref.sh) over an in-memory etcd.
+InstanceMgr::get_load_metrics compiled unmodified from the reference checkout (oracle/build_ref.sh) over an in-memory etcd.
 The restatement (oracle/prefix_oracle.cc, oracle/xxh3_oracle.c) — which every GPU parity test compares the device
 against — must agree with it on the XXH3 known answers, on random block hashes, and on random
-event / upload / match / route histories.  Skipped only where neither /root/reference nor a prebuilt _ref exists."""
+event / upload / match / route histories.  Skipped only where neither the reference checkout nor a prebuilt _ref exists."""
 import json
 import os
 import subprocess
@@ -16,7 +16,7 @@ from oracle import ref
 HERE = os.path.dirname(__file__)
 ROOT = os.path.dirname(HERE)
 
-pytestmark = pytest.mark.skipif(not ref.available(), reason="oracle/_ref not built and /root/reference absent")
+pytestmark = pytest.mark.skipif(not ref.available(), reason="oracle/_ref not built and the reference checkout absent")
 
 
 def test_xxh3_known_answers_and_random_blocks(oracle):

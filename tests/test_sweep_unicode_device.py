@@ -1,6 +1,6 @@
 """Exhaustive device-vs-oracle sweeps over every Unicode code point: all 1.1 M scalar values, each in five contexts
 ("a<c>b <c>1\n<c>"), through the CUDA normaliser / pre-tokenizers / merge kernels against the CPU oracle — 5 models,
-~30 s on a B200, part of `-m gpu` (also selectable alone with `-m sweep`).  The oracles themselves are swept against
+part of `-m gpu` (also selectable alone with `-m sweep`).  The oracles themselves are swept against
 the upstream wheels on CPU (tests/test_oracle_sp.py, tests/test_oracle_hf.py), so this is what separates the device
 tables from the oracle's although both are generated from one Unicode data file."""
 import os

@@ -1,6 +1,6 @@
-"""xllm_service_b200 — B200-native request-ingest + prefix-cache routing path.
+"""xllm_service_b200 — H100-native request-ingest + prefix-cache routing path.
 
-The product is ``libxllm_ingest.so`` (CUDA sm_100a kernels behind the C-ABI of
+The product is ``libxllm_ingest.so`` (CUDA sm_90a kernels behind the C-ABI of
 ``include/xllm_ingest.h``).  This package is the thin Python host-side mirror of
 the reference's operator interfaces for that path (``Tokenizer.encode``,
 ``xxh3_128bits_hash``, ``GlobalKVCacheMgr.match``, ``CacheAwareRouting``) used by

@@ -1,4 +1,4 @@
-// Shared helpers for the ingest kernels (sm_100a only).
+// Shared helpers for the ingest kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -32,7 +32,7 @@ namespace xllm {
 constexpr int kMaxInstances = 64;
 
 // Field order = sector order: key, state and the HBM mask share the first 32-byte sector (what a probe that does not
-// match reads); DRAM still serves the whole 64-byte line, measured (DESIGN.md §6).
+// match reads); DRAM still serves the whole 64-byte line (DESIGN.md §6).
 struct IndexSlot {
   uint64_t klo, khi;
   uint32_t state;  // 0 empty, 1 full, 2 tombstone, 3 busy (claimed by an insert, key not yet visible)

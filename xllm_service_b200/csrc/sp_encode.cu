@@ -1,4 +1,4 @@
-// sp_encode.cu — the batched tokenizer kernels on sm_100a: one warp per request.
+// sp_encode.cu — the batched tokenizer kernels on sm_90a: one warp per request.
 //
 // Bit-exact target: what Tokenizer::encode returns on each of the reference's backends —
 //   SentencePiece (sentencepiece_tokenizer.cpp:115-168 -> sp_processor_.Encode):
@@ -2029,8 +2029,8 @@ __device__ bool drain_pass(const SpDev& T, SM& sm, ReqState& rs, bool final, int
 }
 
 // drain_pass with the warm-up pre-passes (1b below) for natural text — a COPY of drain_pass with them worked in, kept
-// apart because carrying the extra state through the in-order rounds costs the plain kernel 25 % on the headline
-// workload (profiles/r02_experiment_warmup_*): the launcher picks the WARM kernels only when asked to (XLLM_SP_WARM=1).
+// apart because carrying the extra state through the in-order rounds slows the plain kernel on the headline
+// workload: the launcher picks the WARM kernels only when asked to (XLLM_SP_WARM=1).
 template <bool SMALL, bool LONG, int MODE, bool MEMO, typename SM>
 __device__ bool drain_pass_warm(const SpDev& T, SM& sm, ReqState& rs, bool final, int lane, MemoRef memo) {
   constexpr bool HF = MODE == 1;

@@ -1,4 +1,4 @@
-// xxh3_chain.cu — chained per-block XXH3-128 over token-ID streams, sm_100a.
+// xxh3_chain.cu — chained per-block XXH3-128 over token-ID streams, sm_90a.
 //
 // Reference semantics (bit-exact target):
 //   xllm_service/common/hash_util.cpp:18-45            xxh3_128bits_hash

@@ -1,5 +1,5 @@
 // reference_adaptors.h — the reference-side bindings a maintainer drops into xllm-service to put the
-// B200 path behind its existing seams.  It includes the reference's OWN headers (tokenizer/tokenizer.h,
+// H100 path behind its existing seams.  It includes the reference's OWN headers (tokenizer/tokenizer.h,
 // common/slice.h, common/types.h, scheduler/loadbalance_policy/loadbalance_policy.h) and is compiled against them,
 // unmodified, by oracle/build_ref.sh into oracle/_ref/reference_seams_test (tests/cpp/reference_seams_main.cc,
 // run on the GPU by tests/test_gpu_reference_seams.py).  See INTEGRATION.md.
