@@ -248,6 +248,17 @@ __device__ __forceinline__ U128 ld_b128(const void* p) {
                : "=l"(v.lo), "=l"(v.hi) : "l"(p) : "memory");
   return v;
 }
+// The same load without the .relaxed.gpu qualifier, so that the SM's L1 may serve it: the express kernel's memo probes
+// (exp_probe_finish).  An aligned 16-byte load returns one whole 16-byte value that was stored there, possibly an
+// older one than L2 holds, and every value a slot half ever holds gives the exact result: zero or another word's key
+// is a miss (the lane merges the word, and its insert finds the key, when it is already there); the word's key with
+// zero ids is a miss; the word's key with its ids is a hit.  A launch writes each half at most once, from zero.
+__device__ __forceinline__ U128 ld_b128_cached(const void* p) {
+  U128 v;
+  asm volatile("{.reg .b128 t; ld.global.b128 t, [%2]; mov.b128 {%0,%1}, t; }"
+               : "=l"(v.lo), "=l"(v.hi) : "l"(p) : "memory");
+  return v;
+}
 __device__ __forceinline__ void st_b128(void* p, U128 v) {
   asm volatile("{.reg .b128 t; mov.b128 t, {%1,%2}; st.relaxed.gpu.global.b128 [%0], t; }"
                :: "l"(p), "l"(v.lo), "l"(v.hi) : "memory");
@@ -1289,14 +1300,17 @@ __device__ __forceinline__ U128 exp_word_key(const uint4* txt, uint32_t s, int n
   return U128{(lo << 8) | (unsigned long long)((lead ? 0x80u : 0u) | (uint32_t)n), (hi << 8) | (lo >> 56)};
 }
 // The memo probe's second half: compare the first way loaded by the caller, load the second way when the first holds
-// another word.  Returns hit (a key match with ids); val holds the payload of the way that matched.
+// another word.  Returns hit (a key match with ids); val holds the payload of the way that matched.  Both ways are
+// loaded with ld_b128_cached: the hot words' slots stay in the SM's L1, which takes the L2 round trip off most
+// probes, the longest link of a step.  A slot read before another SM's insert reaches it reads as a miss: the lane
+// merges the word, and its insert's CAS, which goes to L2, finds the key there.
 template <bool SMALL>
 __device__ __forceinline__ bool exp_probe_finish(MemoRef memo, U128 key, uint32_t slot, U128 k, U128& val) {
   if (k.lo == key.lo && k.hi == key.hi) return MemoIds<SMALL>::valid(val);
   if ((k.lo | k.hi) == 0) return false;
   const uint8_t* e = memo.table + (size_t)(slot ^ 1u) * 32;
-  const U128 k2 = ld_b128(e);
-  val = ld_b128(e + 16);
+  const U128 k2 = ld_b128_cached(e);
+  val = ld_b128_cached(e + 16);
   return k2.lo == key.lo && k2.hi == key.hi && MemoIds<SMALL>::valid(val);
 }
 // A word's ids from its memo payload at out[o ..]; c1 / c2: some lane of the warp has a word of >= 2 / >= 4 ids.
@@ -1483,12 +1497,12 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
         const uint32_t slotA = memo_slot(keyA, memo.mask), slotB = memo_slot(keyB, memo.mask);
         U128 kA{0ull, 0ull}, kB{0ull, 0ull};
         if (activeA) {
-          kA = ld_b128(memo.table + (size_t)slotA * 32);
-          valA = ld_b128(memo.table + (size_t)slotA * 32 + 16);
+          kA = ld_b128_cached(memo.table + (size_t)slotA * 32);
+          valA = ld_b128_cached(memo.table + (size_t)slotA * 32 + 16);
         }
         if (activeB) {
-          kB = ld_b128(memo.table + (size_t)slotB * 32);
-          valB = ld_b128(memo.table + (size_t)slotB * 32 + 16);
+          kB = ld_b128_cached(memo.table + (size_t)slotB * 32);
+          valB = ld_b128_cached(memo.table + (size_t)slotB * 32 + 16);
         }
         if (activeA) hitA = exp_probe_finish<SMALL>(memo, keyA, slotA, kA, valA);
         if (activeB) hitB = exp_probe_finish<SMALL>(memo, keyB, slotB, kB, valB);
