@@ -20,7 +20,7 @@ VARIANTS = [
     ("off", {"XLLM_SP_MEMO_SLOTS": "0"}),
     ("wide", {"XLLM_SP_FORCE_WIDE": "1"}),
     ("wide_off", {"XLLM_SP_FORCE_WIDE": "1", "XLLM_SP_MEMO_SLOTS": "0"}),
-    # the warm-up kernels (drain_pass_warm: memo misses merged ahead in full rounds, long words resolved ahead into the
+    # the warm-up kernels (drain_pass with WARM: memo misses merged ahead in full rounds, long words resolved ahead into the
     # per-warp scratch), narrow and wide, and with a memo so small that the warm-up's inserts mostly fail
     ("warm", {"XLLM_SP_WARM": "1"}),
     ("warm_wide", {"XLLM_SP_WARM": "1", "XLLM_SP_FORCE_WIDE": "1"}),
@@ -99,7 +99,7 @@ def test_hf_variants(oracle, name, env):
         h.close()
 
 
-@pytest.mark.parametrize("name,env", [VARIANTS[0], VARIANTS[3]])
+@pytest.mark.parametrize("name,env", [VARIANTS[0], VARIANTS[3], VARIANTS[5]])
 def test_tiktoken_variants(oracle, name, env):
     tk = oracle.TiktokenOracle(TK_DIR)
     texts = [t for t in _texts(5)[:40]]

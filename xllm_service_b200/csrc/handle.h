@@ -99,7 +99,7 @@ struct xllm_ingest {
   int64_t memo_persist_requests = 0;  // 0: every launch clears its memo; N > 0: a memo is kept until it has seen N requests
   xllm::DevBuf d_arena;     // warm-up scratch of the encode kernel (per handle: launches on one handle are serialised)
   uint32_t memo_slots = 0;  // 0 = memo off
-  bool sp_warm = false;     // XLLM_SP_WARM=1: launch the warm-up tokenizer kernels (natural text; sp_encode.cu drain_pass_warm)
+  bool sp_warm = false;     // XLLM_SP_WARM=1: launch the warm-up tokenizer kernels (natural text; sp_encode.cu drain_pass, WARM)
   xllm::DevBuf d_tokens, d_tok_start, d_n_tok, d_keys, d_key_start;
   // sharded xllm_ingest_batch: the whole batch's keys / row descriptors / results stay resident for the one exchange
   xllm::DevBuf d_all_keys, d_all_key_start, d_all_n_blocks, d_all_match, d_all_routing;

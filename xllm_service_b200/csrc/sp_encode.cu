@@ -926,9 +926,6 @@ __device__ __noinline__ bool long_enter(const SpDev& T, SM& sm, ReqState& rs, in
   return true;
 }
 
-// Tokenises the complete words held in nbuf (all words when final) and keeps the incomplete tail.
-// HF: word boundaries come from the regex pre-tokenizer (hf_pretok.cuh); returns true when the word list
-// filled up and the kept tail has to be scanned again.
 #ifdef XLLM_MEMO_STATS
 __device__ unsigned long long g_memo_stats[8];
 #endif
@@ -1691,414 +1688,39 @@ __global__ void __launch_bounds__(kExpWarps * 32, XLLM_EXP_MIN_BLOCKS) sp_expres
   }
 }
 
-// MODE: 0 SentencePiece BPE / tiktoken, 1 HF byte-level BPE (regex pre-tokenizer), 2 SentencePiece Unigram
-template <bool SMALL, bool LONG, int MODE, bool MEMO, typename SM>
-__device__ bool drain_pass(const SpDev& T, SM& sm, ReqState& rs, bool final, int lane, MemoRef memo) {
-  constexpr bool HF = MODE == 1;
-  constexpr bool UNI = MODE == 2;
+// Writes the symbols of the chars of nbuf[ws, we) flat to S[0..n) and returns n.  *overflow (the same in every lane):
+// the word has more than kCoopMaxSym chars, and S holds only the first of them.
+template <typename SM>
+__device__ __forceinline__ int gather_chars(const SpDev& T, SM& sm, int ws, int we, bool* overflow, int lane) {
   const uint8_t* nb = sm.nbuf;
-  int nlen = rs.nlen;
-  if (final && T.remove_extra_ws) {
-    // normalizer.cc: "Ignores trailing space" — strip trailing U+2581 from the stream
-    while (nlen >= 3 && nb[nlen - 3] == 0xE2 && nb[nlen - 2] == 0x96 && nb[nlen - 1] == 0x81) nlen -= 3;
-    if (nlen == 0) { rs.n_out -= rs.trailing_bare; rs.trailing_bare = 0; }
-  }
-  if (nlen == 0) { rs.nlen = 0; return false; }
-
-  // 1. word starts: recorded by the fast path, or re-derived after any general-path window
-  int nwords = 0;
-  int hf_tail = 0;
-  bool hf_capped = false;
-  if constexpr (HF) {
-    const HfScan sc = hf_scan(T, sm, nlen, final, lane);
-    if (sc.bad) { rs.bad_input = (int8_t)sc.bad; return false; }
-    nwords = sc.nwords;
-    hf_tail = sc.tail_start;
-    hf_capped = sc.capped;
-  } else if (!rs.rescan && !(final && nlen != rs.nlen)) {
-    nwords = rs.nw;
-  } else if (!rs.rescan) {
-    // trailing U+2581 were stripped: drop the starts that now lie at or past the end
-    nwords = rs.nw;
-    while (nwords > 1 && sm.wstart[nwords - 1] >= nlen) --nwords;
-  } else {
-    for (int base = 0; base < nlen; base += 32) {
-      const int p = base + lane;
-      bool st = false;
-      if (p < nlen) {
-        if (p == 0) st = true;
-        else if (T.split_mode != 0 && is_space_at(nb, p, nlen)) {
-          st = T.split_mode == 1 || !(p >= 3 && is_space_at(nb, p - 3, nlen));
-        }
-      }
-      const uint32_t m = __ballot_sync(kFull, st);
-      if (st) sm.wstart[nwords + __popc(m & ((1u << lane) - 1))] = (uint16_t)p;
-      nwords += __popc(m);
+  int n = 0;
+  bool over = false;
+  for (int base = ws; base < we; base += 32) {
+    const int p = base + lane;
+    const bool lead = p < we && (T.byte_mode || (nb[p] & 0xC0) != 0x80);
+    const uint32_t m = __ballot_sync(kFull, lead);
+    const int idx = n + __popc(m & ((1u << lane) - 1));
+    if (lead) {
+      if (idx < kCoopMaxSym) { uint32_t adv; sm.S[idx] = char_sym(T, nb + p, &adv); }
+      else over = true;
     }
+    n += __popc(m);
   }
+  *overflow = __any_sync(kFull, over);
   __syncwarp();
-  if constexpr (!HF) {
-    if (lane == 0) sm.wstart[nwords] = (uint16_t)nlen;
-    __syncwarp();
-  }
-  const int complete = HF ? nwords : (final ? nwords : nwords - 1);
-
-  // 2. rounds of up to 32 consecutive words
-  int w0 = 0;
-  while (w0 < complete && !rs.deferred) {
-    const int w = w0 + lane;
-    const bool have = w < complete;
-    int ws = 0, we = 0, nsym = 0;
-    bool special = false;  // HF: the word is an added token
-    if constexpr (HF) {
-      if (have) {
-        const uint16_t e = sm.wstart[w];
-        ws = e & kHfPosMask;
-        we = sm.wstart[w + 1] & kHfPosMask;
-        special = (e & kHfSpecialWord) != 0;
-        nsym = special ? 1 : we - ws;  // every byte is a symbol
-      }
-    } else if (have) {
-      ws = sm.wstart[w];
-      we = sm.wstart[w + 1];
-      if (rs.ascii) nsym = (we - ws) - (nb[ws] == 0xE2 ? 2 : 0);  // ASCII + one leading U+2581
-      else
-        for (int p = ws; p < we; ++p) nsym += T.byte_mode || (nb[p] & 0xC0) != 0x80;
-    }
-    const uint32_t long_mask = __ballot_sync(kFull, have && (UNI || nsym > SM::kRows));  // Unigram: one word at a time
-    const int first_long = long_mask ? __ffs(long_mask) - 1 : 32;
-    const bool active = have && lane < first_long;
-
-    // --- fast path: one word per lane
-    uint32_t alive = 0;
-    int cnt = 0;
-    bool first_unk = false, last_unk = false, bare = false;
-    bool memo_hit = false;
-    if constexpr (MEMO) {
-      U128 key;
-      if (active && !special && memo_key(nb, ws, we, T.byte_mode, &key)) {
-        uint32_t slot = memo_slot(key, memo.mask);
-#pragma unroll 1
-        for (int way = 0; way < 2; ++way, slot ^= 1u) {
-          const uint8_t* e = memo.table + (size_t)slot * 32;
-          const U128 k = ld_b128(e);
-          const U128 v = ld_b128(e + 16);
-          if (k.lo == key.lo && k.hi == key.hi) {
-            if (MemoIds<SMALL>::valid(v)) {
-              memo_hit = true;
-              cnt = MemoIds<SMALL>::count(v);
-              alive = (1u << cnt) - 1u;
-#pragma unroll
-              for (int q = 0; q < MemoIds<SMALL>::kMax; ++q)
-                if (q < cnt) sm.S[q * 32 + lane] = kResolvedFlag | MemoIds<SMALL>::id(v, q);
-            }
-            break;
-          }
-          if ((k.lo | k.hi) == 0) break;  // empty: the word was not seen yet
-        }
-      }
-    }
-#ifdef XLLM_MEMO_STATS
-    {
-      const uint32_t am = __ballot_sync(kFull, active), hm = __ballot_sync(kFull, memo_hit);
-      if (lane == 0) {
-        atomicAdd(&g_memo_stats[0], 1ull);                       // rounds
-        atomicAdd(&g_memo_stats[1], (unsigned long long)__popc(am));   // active words
-        atomicAdd(&g_memo_stats[2], (unsigned long long)__popc(hm));   // hits
-        if (am & ~hm) atomicAdd(&g_memo_stats[3], 1ull);         // rounds with a slow-path lane
-        if (first_long < 32) atomicAdd(&g_memo_stats[4], 1ull);  // rounds cut by a long word
-      }
-    }
-#endif
-    if (memo_hit) {
-    } else if (HF && active && special) {
-      int32_t id = 0;
-      hf_added_len(T, nb + ws, we - ws, &id);
-      sm.S[lane] = kResolvedFlag | (uint32_t)id;
-      alive = 1u;
-      cnt = 1;
-    } else if (active) {
-      bool direct = false;
-      if constexpr (HF) {
-        if (T.ignore_merges) {  // models/bpe/model.rs: a pre-token that is a vocabulary entry is that token
-          const int32_t id = hf_vocab_lookup(T, nb + ws, we - ws);
-          if (id >= 0) {
-            sm.S[lane] = kResolvedFlag | (uint32_t)id;
-            alive = 1u;
-            cnt = 1;
-            direct = true;
-          }
-        }
-      }
-      bool pu = false, first = true;
-      if (!direct) {
-        int n = 0;
-        for (int p = ws; p < we;) {
-          uint32_t adv;
-          sm.S[n * 32 + lane] = char_sym(T, nb + p, &adv);
-          p += adv;
-          ++n;
-        }
-        bare = (we - ws == 3) && n == 1 && sm.S[lane] == T.space_sym;
-        alive = lane_merge<SMALL>(T, sm, n, lane);
-      }
-      // pass 1: resolve every final symbol; single-id symbols are replaced in place by their token id
-      // (tagged), so pass 2 only re-derives the rare multi-id (byte fallback) ones
-      for (uint32_t m = direct ? 0u : alive; m;) {
-        const int j = __ffs(m) - 1;
-        m &= m - 1;
-        int32_t tmp[4];
-        bool unk;
-        const uint32_t sym = sm.S[j * 32 + lane];
-        const int c = sym_ids(T, sym, tmp, &unk);
-        if (first) { first_unk = unk; first = false; }
-        if (!unk && c == 1) sm.S[j * 32 + lane] = kResolvedFlag | (uint32_t)tmp[0];
-        if (!(unk && pu && !T.byte_fallback)) cnt += c;
-        pu = unk;
-      }
-      last_unk = pu;
-      if constexpr (MEMO) {
-        // memoise: every surviving symbol resolved to exactly one id, at most four of them
-        const int k = __popc(alive);
-        U128 key;
-        if (k >= 1 && k <= MemoIds<SMALL>::kMax && k == cnt && !bare && memo_key(nb, ws, we, T.byte_mode, &key)) {
-          uint32_t id[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-          bool ok = true;
-          int q = 0;
-          for (uint32_t m = alive; m; ++q) {
-            const int j = __ffs(m) - 1;
-            m &= m - 1;
-            const uint32_t sym = sm.S[j * 32 + lane];
-            ok = ok && (sym & 0xC0000000u) == kResolvedFlag && (sym & 0x3FFFFFFFu) < (SMALL ? (1u << 16) : (1u << 28));
-            id[q] = sym & 0x0FFFFFFFu;
-          }
-          if (ok) {
-            const U128 val = MemoIds<SMALL>::pack(k, id);
-            uint32_t slot = memo_slot(key, memo.mask);
-            const U128 zero{0ull, 0ull};
-#pragma unroll 1
-            for (int way = 0; way < 2; ++way, slot ^= 1u) {
-              uint8_t* e = memo.table + (size_t)slot * 32;
-              const U128 old = cas_b128(e, zero, key);
-              if ((old.lo | old.hi) == 0) { st_b128(e + 16, val); break; }   // claimed: publish the ids
-              if (old.lo == key.lo && old.hi == key.hi) break;                // another warp owns this word
-            }
-          }
-        }
-      }
-    }
-    // cross-word unknown merging (byte_fallback off): drop the first id if the previous symbol was unknown too
-    bool drop_first = false;
-    if (!T.byte_fallback) {
-      const uint32_t act_mask = __ballot_sync(kFull, active);
-      const uint32_t lu_mask = __ballot_sync(kFull, active && last_unk);
-      if (active && first_unk) {
-        const bool prev = lane == 0 ? rs.prev_unk : ((lu_mask >> (lane - 1)) & 1u);
-        if (prev) { drop_first = true; cnt -= 1; }
-      }
-      if (act_mask) rs.prev_unk = (lu_mask >> (31 - __clz(act_mask))) & 1u;
-    }
-    const int incl = warp_incl_scan(cnt, lane);
-    const int total = __shfl_sync(kFull, incl, 31);
-    if (active) {
-      int64_t o = rs.n_out + (incl - cnt);
-      bool pu = false, first = true;
-      for (uint32_t m = alive; m;) {
-        const int j = __ffs(m) - 1;
-        m &= m - 1;
-        const uint32_t sym = sm.S[j * 32 + lane];
-        if ((sym & 0xC0000000u) == kResolvedFlag) {  // known symbol: one id
-          put_id(rs, o++, (int32_t)(sym & 0x3FFFFFFFu));
-          pu = false;
-        } else {
-          int32_t tmp[4];
-          bool unk;
-          const int c = sym_ids(T, sym, tmp, &unk);
-          const bool skip = (unk && pu && !T.byte_fallback) || (first && drop_first);
-          if (!skip)
-            for (int k = 0; k < c; ++k) put_id(rs, o++, tmp[k]);
-          pu = unk;
-        }
-        first = false;
-      }
-    }
-    rs.n_out += total;
-    // trailing bare-word bookkeeping: ids of the run of bare words at the end of what was emitted
-    {
-      const uint32_t act_mask = __ballot_sync(kFull, active);
-      const uint32_t nonbare = __ballot_sync(kFull, active && !bare);
-      if (act_mask) {
-        const int last_nb = nonbare ? 31 - __clz(nonbare) : -1;  // last non-bare lane
-        const int tail = __shfl_sync(kFull, incl, 31) - (last_nb >= 0 ? __shfl_sync(kFull, incl, last_nb) : 0);
-        rs.trailing_bare = (last_nb >= 0 ? 0 : rs.trailing_bare) + tail;
-      }
-    }
-    __syncwarp();
-    w0 += first_long < 32 ? first_long : 32;
-    if (w0 >= complete || first_long == 32) continue;
-
-    // --- cooperative path for the long word w0
-    {
-      const int lws = HF ? (sm.wstart[w0] & kHfPosMask) : sm.wstart[w0];
-      int lwe = HF ? (sm.wstart[w0 + 1] & kHfPosMask) : sm.wstart[w0 + 1];
-      int n = 0;
-      int words_taken = 1;
-      bool overflow = false;
-      bool uni_done = false;
-      if constexpr (UNI) {
-        auto is_bare = [&](int a, int b) { return b - a == 3 && nb[a] == 0xE2 && nb[a + 1] == 0x96 && nb[a + 2] == 0x81; };
-        const bool bare_word = is_bare(lws, lwe);
-        // No piece spans a word start, so consecutive words form one lattice: take as many complete words as the
-        // lattice scratch holds — the trie walks then fill all 32 lanes and the per-word overhead is paid once per run.
-        // A bare U+2581 word stays on its own (trailing-space bookkeeping).
-        if (!bare_word) {
-          while (w0 + words_taken < complete) {
-            const int a = sm.wstart[w0 + words_taken], b = sm.wstart[w0 + words_taken + 1];
-            if (b - lws > kUniMaxWord || is_bare(a, b)) break;
-            lwe = b;
-            ++words_taken;
-          }
-        }
-        const int len = lwe - lws;
-        if (len > kUniMaxWord) {
-          rs.too_long = true;  // the Viterbi lattice of one word lives in shared memory
-        } else {
-          n = unigram_word(T, sm, nb + lws, len, &rs.uni_score, lane);
-          const int64_t before = rs.n_out;
-          for (int base = 0; base < n; base += 32) {
-            const int j = base + lane;
-            int32_t tmp[4];
-            bool unk = false;
-            int c = 0;
-            if (j < n) {
-              const uint32_t sym = sm.S[j];
-              if ((sym & 0xC0000000u) == kResolvedFlag) { tmp[0] = (int32_t)(sym & 0x3FFFFFFFu); c = 1; }
-              else c = sym_ids(T, sym, tmp, &unk);
-            }
-            bool skip = false;
-            if (!T.byte_fallback) {
-              const uint32_t um = __ballot_sync(kFull, j < n && unk);
-              const bool prev = lane == 0 ? rs.prev_unk : ((um >> (lane - 1)) & 1u);
-              skip = unk && prev;
-              const int lastl = (n - base) >= 32 ? 31 : (n - base - 1);
-              rs.prev_unk = (um >> lastl) & 1u;
-            }
-            if (skip) c = 0;
-            const int inc2 = warp_incl_scan(c, lane);
-            int64_t o = rs.n_out + (inc2 - c);
-            for (int k = 0; k < c; ++k) put_id(rs, o++, tmp[k]);
-            rs.n_out += __shfl_sync(kFull, inc2, 31);
-          }
-          rs.trailing_bare = bare_word ? rs.trailing_bare + (int32_t)(rs.n_out - before) : 0;
-        }
-        uni_done = true;
-      }
-      for (int base = lws; base < lwe && !uni_done; base += 32) {
-        const int p = base + lane;
-        const bool lead = p < lwe && (T.byte_mode || (nb[p] & 0xC0) != 0x80);
-        const uint32_t m = __ballot_sync(kFull, lead);
-        const int idx = n + __popc(m & ((1u << lane) - 1));
-        if (lead) {
-          if (idx < kCoopMaxSym) { uint32_t adv; sm.S[idx] = char_sym(T, nb + p, &adv); }
-          else overflow = true;
-        }
-        n += __popc(m);
-      }
-      overflow = __any_sync(kFull, overflow);
-      __syncwarp();
-      int32_t whole = -1;
-      if constexpr (HF) {
-        if (T.ignore_merges && !overflow) {  // no vocabulary entry is longer than the cooperative path (host check)
-          if (lane == 0) whole = hf_vocab_lookup(T, nb + lws, lwe - lws);
-          whole = __shfl_sync(kFull, whole, 0);
-        }
-      }
-      if (uni_done) {
-      } else if (whole >= 0) {
-        if (lane == 0) put_id(rs, rs.n_out, whole);
-        rs.n_out += 1;
-        rs.trailing_bare = 0;
-      } else if (overflow) {
-        // more chars than the shared-memory scratch holds: merge it in a global scratch slot
-        if constexpr (!LONG) {
-          rs.deferred = true;
-        } else if (T.long_slots <= 0) {
-          rs.too_long = true;
-        } else {
-          rs.long_slot = long_slot_acquire(T.long_locks, T.long_slots, lane);
-          rs.long_n = 0;
-          if (long_append(T, sm, rs, lws, lwe, lane)) long_finish(T, rs, false, lane);
-          else rs.too_long = true;
-          long_slot_release(T.long_locks, rs.long_slot, lane);
-        }
-      } else {
-        n = coop_merge<SMALL>(T, sm, n, lane);
-        for (int base = 0; base < n; base += 32) {
-          const int j = base + lane;
-          int32_t tmp[4];
-          bool unk = false;
-          int c = 0;
-          if (j < n) c = sym_ids(T, sm.S[j], tmp, &unk);
-          bool skip = false;
-          if (!T.byte_fallback) {
-            const uint32_t um = __ballot_sync(kFull, j < n && unk);
-            const bool prev = lane == 0 ? rs.prev_unk : ((um >> (lane - 1)) & 1u);
-            skip = unk && prev;
-            const int lastl = (n - base) >= 32 ? 31 : (n - base - 1);
-            rs.prev_unk = (um >> lastl) & 1u;
-          }
-          if (skip) c = 0;
-          const int inc2 = warp_incl_scan(c, lane);
-          int64_t o = rs.n_out + (inc2 - c);
-          for (int k = 0; k < c; ++k) put_id(rs, o++, tmp[k]);
-          rs.n_out += __shfl_sync(kFull, inc2, 31);
-        }
-        rs.trailing_bare = 0;
-      }
-      __syncwarp();
-      w0 += words_taken;
-    }
-  }
-
-  // 3. keep the incomplete tail at the front of nbuf
-  if (!final || (HF && hf_tail < nlen)) {
-    const int ts = HF ? hf_tail : sm.wstart[nwords - 1];
-    const int tl = nlen - ts;
-    if (ts > 0) {
-      for (int base = 0; base < tl; base += 32) {
-        const int k = base + lane;
-        uint8_t c = 0;
-        if (k < tl) c = sm.nbuf[ts + k];
-        __syncwarp();
-        if (k < tl) sm.nbuf[k] = c;
-        __syncwarp();
-      }
-    }
-    rs.nlen = tl;
-    __syncwarp();  // every lane has read wstart[nwords - 1] (which is wstart[0] when one word is left)
-    if (lane == 0) sm.wstart[0] = 0;
-    rs.nw = 1;
-    if (!rs.ascii) {  // the kept tail decides whether the buffer is ASCII-only again
-      bool non_ascii = false;
-      const bool lead = tl >= 3 && sm.nbuf[0] == 0xE2 && sm.nbuf[1] == 0x96 && sm.nbuf[2] == 0x81;
-      for (int k = lane; k < tl; k += 32) non_ascii |= sm.nbuf[k] >= 0x80 && !(lead && k < 3);
-      rs.ascii = !T.byte_mode && !__any_sync(kFull, non_ascii);
-    }
-  } else {
-    rs.nlen = 0;
-    rs.nw = 0;
-    rs.ascii = !T.byte_mode;
-  }
-  rs.rescan = false;
-  __syncwarp();
-  return HF && hf_capped && !rs.deferred;
+  return n;
 }
 
-// drain_pass with the warm-up pre-passes (1b below) for natural text — a COPY of drain_pass with them worked in, kept
-// apart because carrying the extra state through the in-order rounds slows the plain kernel on the headline
-// workload: the launcher picks the WARM kernels only when asked to (XLLM_SP_WARM=1).
-template <bool SMALL, bool LONG, int MODE, bool MEMO, typename SM>
-__device__ bool drain_pass_warm(const SpDev& T, SM& sm, ReqState& rs, bool final, int lane, MemoRef memo) {
+// Tokenises the complete words held in nbuf (all words when final) and keeps the incomplete tail.
+// HF: word boundaries come from the regex pre-tokenizer (hf_pretok.cuh); returns true when the word list
+// filled up and the kept tail has to be scanned again.
+// MODE: 0 SentencePiece BPE / tiktoken, 1 HF byte-level BPE (regex pre-tokenizer), 2 SentencePiece Unigram
+// WARM: with the warm-up pre-passes (1b below) for natural text.  A template parameter because carrying their state
+// through the in-order rounds slows the plain kernel on the headline workload: the launcher picks the WARM kernels
+// only when asked to (XLLM_SP_WARM=1).
+template <bool SMALL, bool LONG, int MODE, bool MEMO, bool WARM, typename SM>
+__device__ bool drain_pass(const SpDev& T, SM& sm, ReqState& rs, bool final, int lane, MemoRef memo) {
+  static_assert(!WARM || (MEMO && !LONG && MODE != 2), "the warm-up pre-passes need the memo and the lane path");
   constexpr bool HF = MODE == 1;
   constexpr bool UNI = MODE == 2;
   const uint8_t* nb = sm.nbuf;
@@ -2166,22 +1788,13 @@ __device__ bool drain_pass_warm(const SpDev& T, SM& sm, ReqState& rs, bool final
         for (int p = ws; p < we; ++p) nsym += T.byte_mode || (nb[p] & 0xC0) != 0x80;
     }
   };
-  // The merge path of one word per lane: symbols -> lane_merge -> resolve single-id symbols in place -> (MEMO) insert.
-  // Used by the rounds below for memo misses and by the warm-up pre-pass.  Outputs: alive set in the lane's S column,
-  // id count, unknown-symbol flags for the cross-word rule, bare-U+2581 flag.
-  auto merge_word = [&](int ws, int we, bool special, uint32_t& alive, int& cnt, bool& first_unk, bool& last_unk,
-                        bool& bare) {
+  // The merge path of one word per lane (not an added token): symbols -> lane_merge -> resolve single-id symbols in
+  // place -> (MEMO) insert.  Used by the rounds below for memo misses and by the warm-up pre-pass.  Outputs: alive set
+  // in the lane's S column, id count, unknown-symbol flags for the cross-word rule, bare-U+2581 flag.
+  auto merge_word = [&](int ws, int we, uint32_t& alive, int& cnt, bool& first_unk, bool& last_unk, bool& bare) {
     alive = 0;
     cnt = 0;
     first_unk = last_unk = bare = false;
-    if (HF && special) {
-      int32_t id = 0;
-      hf_added_len(T, nb + ws, we - ws, &id);
-      sm.S[lane] = kResolvedFlag | (uint32_t)id;
-      alive = 1u;
-      cnt = 1;
-      return;
-    }
     bool direct = false;
     if constexpr (HF) {
       if (T.ignore_merges) {  // models/bpe/model.rs: a pre-token that is a vocabulary entry is that token
@@ -2266,7 +1879,7 @@ __device__ bool drain_pass_warm(const SpDev& T, SM& sm, ReqState& rs, bool final
   int32_t* arena = nullptr;
   uint16_t* lcnt = nullptr;
   int a1_misses = 0;
-  if constexpr (MEMO && !UNI && !LONG) {
+  if constexpr (WARM) {
     if (T.warm_arena != nullptr && (rs.warm || rs.had_long)) {
       uint8_t* slice = T.warm_arena + (size_t)blockIdx.x * kWarmSliceBytes;
       const bool do_long = rs.had_long && (T.byte_fallback || T.byte_mode);
@@ -2283,7 +1896,7 @@ __device__ bool drain_pass_warm(const SpDev& T, SM& sm, ReqState& rs, bool final
         uint32_t alive;
         int cnt;
         bool fu, lu, bare;
-        if (lane < np) merge_word(ws, we, special, alive, cnt, fu, lu, bare);
+        if (lane < np) merge_word(ws, we, alive, cnt, fu, lu, bare);   // A1 never holds an added token
         np = 0;
         __syncwarp();
       };
@@ -2293,28 +1906,15 @@ __device__ bool drain_pass_warm(const SpDev& T, SM& sm, ReqState& rs, bool final
         int ws = 0, we = 0, nsym = 0;
         bool special = false;
         if (have) word_of(w, ws, we, nsym, special);
-        const bool is_long = have && !special && nsym > kMaxSym;
+        const bool is_long = have && !special && nsym > SM::kRows;
         // ---- A2: the long words of this block, one at a time, whole warp
         uint32_t lm = __ballot_sync(kFull, do_long && is_long);
         while (lm) {
           const int b = __ffs(lm) - 1;
           lm &= lm - 1;
           const int lws = __shfl_sync(kFull, ws, b), lwe = __shfl_sync(kFull, we, b);
-          int n = 0;
-          bool overflow = false;
-          for (int pb = lws; pb < lwe; pb += 32) {
-            const int p = pb + lane;
-            const bool lead = p < lwe && (T.byte_mode || (nb[p] & 0xC0) != 0x80);
-            const uint32_t m = __ballot_sync(kFull, lead);
-            const int idx = n + __popc(m & ((1u << lane) - 1));
-            if (lead) {
-              if (idx < kCoopMaxSym) { uint32_t adv; sm.S[idx] = char_sym(T, nb + p, &adv); }
-              else overflow = true;
-            }
-            n += __popc(m);
-          }
-          overflow = __any_sync(kFull, overflow);
-          __syncwarp();
+          bool overflow;
+          int n = gather_chars(T, sm, lws, lwe, &overflow, lane);
           int total = -1;   // ids written for this word, -1: left to the in-order cooperative path
           if (!overflow) {
             int32_t whole = -1;
@@ -2386,11 +1986,9 @@ __device__ bool drain_pass_warm(const SpDev& T, SM& sm, ReqState& rs, bool final
     if (have) word_of(w, ws, we, nsym, special);
     // a long word the pre-pass resolved: its ids wait in the arena, it takes part in the round like any other lane
     bool pre = false;
-    if constexpr (MEMO && !UNI && !LONG) {
-      pre = arena != nullptr && have && !special && nsym > kMaxSym && lcnt[w] != kNotPre;
-    }
-    const uint32_t long_mask = __ballot_sync(kFull, have && (UNI || (nsym > kMaxSym && !pre)));  // Unigram: one word at a time
-    long_seen |= long_mask != 0 || __any_sync(kFull, pre);
+    if constexpr (WARM) pre = arena != nullptr && have && !special && nsym > SM::kRows && lcnt[w] != kNotPre;
+    const uint32_t long_mask = __ballot_sync(kFull, have && (UNI || (nsym > SM::kRows && !pre)));  // Unigram: one word at a time
+    if constexpr (WARM) long_seen |= long_mask != 0 || __any_sync(kFull, pre);
     const int first_long = long_mask ? __ffs(long_mask) - 1 : 32;
     const bool active = have && lane < first_long;
 
@@ -2437,10 +2035,19 @@ __device__ bool drain_pass_warm(const SpDev& T, SM& sm, ReqState& rs, bool final
 #endif
     if (pre && active) {
       cnt = lcnt[w];   // ids parked in the arena by the pre-pass (byte fallback / byte level: no unknown merging)
-    } else if (!memo_hit && active) {
-      merge_word(ws, we, special, alive, cnt, first_unk, last_unk, bare);
+    } else if (memo_hit) {
+    } else if (HF && active && special) {
+      int32_t id = 0;
+      hf_added_len(T, nb + ws, we - ws, &id);
+      sm.S[lane] = kResolvedFlag | (uint32_t)id;
+      alive = 1u;
+      cnt = 1;
+    } else if (active) {
+      merge_word(ws, we, alive, cnt, first_unk, last_unk, bare);
     }
-    if (__any_sync(kFull, active && !pre && !memo_hit && !special)) ++n_slow;
+    if constexpr (WARM) {
+      if (__any_sync(kFull, active && !pre && !memo_hit && !special)) ++n_slow;
+    }
     // cross-word unknown merging (byte_fallback off): drop the first id if the previous symbol was unknown too
     bool drop_first = false;
     if (!T.byte_fallback) {
@@ -2498,10 +2105,7 @@ __device__ bool drain_pass_warm(const SpDev& T, SM& sm, ReqState& rs, bool final
     {
       const int lws = HF ? (sm.wstart[w0] & kHfPosMask) : sm.wstart[w0];
       int lwe = HF ? (sm.wstart[w0 + 1] & kHfPosMask) : sm.wstart[w0 + 1];
-      int n = 0;
       int words_taken = 1;
-      bool overflow = false;
-      bool uni_done = false;
       if constexpr (UNI) {
         auto is_bare = [&](int a, int b) { return b - a == 3 && nb[a] == 0xE2 && nb[a + 1] == 0x96 && nb[a + 2] == 0x81; };
         const bool bare_word = is_bare(lws, lwe);
@@ -2520,7 +2124,7 @@ __device__ bool drain_pass_warm(const SpDev& T, SM& sm, ReqState& rs, bool final
         if (len > kUniMaxWord) {
           rs.too_long = true;  // the Viterbi lattice of one word lives in shared memory
         } else {
-          n = unigram_word(T, sm, nb + lws, len, &rs.uni_score, lane);
+          const int n = unigram_word(T, sm, nb + lws, len, &rs.uni_score, lane);
           const int64_t before = rs.n_out;
           for (int base = 0; base < n; base += 32) {
             const int j = base + lane;
@@ -2548,69 +2152,57 @@ __device__ bool drain_pass_warm(const SpDev& T, SM& sm, ReqState& rs, bool final
           }
           rs.trailing_bare = bare_word ? rs.trailing_bare + (int32_t)(rs.n_out - before) : 0;
         }
-        uni_done = true;
-      }
-      for (int base = lws; base < lwe && !uni_done; base += 32) {
-        const int p = base + lane;
-        const bool lead = p < lwe && (T.byte_mode || (nb[p] & 0xC0) != 0x80);
-        const uint32_t m = __ballot_sync(kFull, lead);
-        const int idx = n + __popc(m & ((1u << lane) - 1));
-        if (lead) {
-          if (idx < kCoopMaxSym) { uint32_t adv; sm.S[idx] = char_sym(T, nb + p, &adv); }
-          else overflow = true;
-        }
-        n += __popc(m);
-      }
-      overflow = __any_sync(kFull, overflow);
-      __syncwarp();
-      int32_t whole = -1;
-      if constexpr (HF) {
-        if (T.ignore_merges && !overflow) {  // no vocabulary entry is longer than the cooperative path (host check)
-          if (lane == 0) whole = hf_vocab_lookup(T, nb + lws, lwe - lws);
-          whole = __shfl_sync(kFull, whole, 0);
-        }
-      }
-      if (uni_done) {
-      } else if (whole >= 0) {
-        if (lane == 0) put_id(rs, rs.n_out, whole);
-        rs.n_out += 1;
-        rs.trailing_bare = 0;
-      } else if (overflow) {
-        // more chars than the shared-memory scratch holds: merge it in a global scratch slot
-        if constexpr (!LONG) {
-          rs.deferred = true;
-        } else if (T.long_slots <= 0) {
-          rs.too_long = true;
-        } else {
-          rs.long_slot = long_slot_acquire(T.long_locks, T.long_slots, lane);
-          rs.long_n = 0;
-          if (long_append(T, sm, rs, lws, lwe, lane)) long_finish(T, rs, false, lane);
-          else rs.too_long = true;
-          long_slot_release(T.long_locks, rs.long_slot, lane);
-        }
       } else {
-        n = coop_merge<SMALL>(T, sm, n, lane);
-        for (int base = 0; base < n; base += 32) {
-          const int j = base + lane;
-          int32_t tmp[4];
-          bool unk = false;
-          int c = 0;
-          if (j < n) c = sym_ids(T, sm.S[j], tmp, &unk);
-          bool skip = false;
-          if (!T.byte_fallback) {
-            const uint32_t um = __ballot_sync(kFull, j < n && unk);
-            const bool prev = lane == 0 ? rs.prev_unk : ((um >> (lane - 1)) & 1u);
-            skip = unk && prev;
-            const int lastl = (n - base) >= 32 ? 31 : (n - base - 1);
-            rs.prev_unk = (um >> lastl) & 1u;
+        bool overflow;
+        int n = gather_chars(T, sm, lws, lwe, &overflow, lane);
+        int32_t whole = -1;
+        if constexpr (HF) {
+          if (T.ignore_merges && !overflow) {  // no vocabulary entry is longer than the cooperative path (host check)
+            if (lane == 0) whole = hf_vocab_lookup(T, nb + lws, lwe - lws);
+            whole = __shfl_sync(kFull, whole, 0);
           }
-          if (skip) c = 0;
-          const int inc2 = warp_incl_scan(c, lane);
-          int64_t o = rs.n_out + (inc2 - c);
-          for (int k = 0; k < c; ++k) put_id(rs, o++, tmp[k]);
-          rs.n_out += __shfl_sync(kFull, inc2, 31);
         }
-        rs.trailing_bare = 0;
+        if (whole >= 0) {
+          if (lane == 0) put_id(rs, rs.n_out, whole);
+          rs.n_out += 1;
+          rs.trailing_bare = 0;
+        } else if (overflow) {
+          // more chars than the shared-memory scratch holds: merge it in a global scratch slot
+          if constexpr (!LONG) {
+            rs.deferred = true;
+          } else if (T.long_slots <= 0) {
+            rs.too_long = true;
+          } else {
+            rs.long_slot = long_slot_acquire(T.long_locks, T.long_slots, lane);
+            rs.long_n = 0;
+            if (long_append(T, sm, rs, lws, lwe, lane)) long_finish(T, rs, false, lane);
+            else rs.too_long = true;
+            long_slot_release(T.long_locks, rs.long_slot, lane);
+          }
+        } else {
+          n = coop_merge<SMALL>(T, sm, n, lane);
+          for (int base = 0; base < n; base += 32) {
+            const int j = base + lane;
+            int32_t tmp[4];
+            bool unk = false;
+            int c = 0;
+            if (j < n) c = sym_ids(T, sm.S[j], tmp, &unk);
+            bool skip = false;
+            if (!T.byte_fallback) {
+              const uint32_t um = __ballot_sync(kFull, j < n && unk);
+              const bool prev = lane == 0 ? rs.prev_unk : ((um >> (lane - 1)) & 1u);
+              skip = unk && prev;
+              const int lastl = (n - base) >= 32 ? 31 : (n - base - 1);
+              rs.prev_unk = (um >> lastl) & 1u;
+            }
+            if (skip) c = 0;
+            const int inc2 = warp_incl_scan(c, lane);
+            int64_t o = rs.n_out + (inc2 - c);
+            for (int k = 0; k < c; ++k) put_id(rs, o++, tmp[k]);
+            rs.n_out += __shfl_sync(kFull, inc2, 31);
+          }
+          rs.trailing_bare = 0;
+        }
       }
       __syncwarp();
       w0 += words_taken;
@@ -2647,7 +2239,7 @@ __device__ bool drain_pass_warm(const SpDev& T, SM& sm, ReqState& rs, bool final
     rs.ascii = !T.byte_mode;
   }
   rs.rescan = false;
-  if constexpr (MEMO && !UNI && !LONG) {
+  if constexpr (WARM) {
     // the next drain of this request (and, carried over, the next request of the batch) warms up when this one paid
     // for misses, and resolves long words ahead when this one had any
     rs.warm = n_slow >= 2 || a1_misses >= 8;
@@ -2657,18 +2249,12 @@ __device__ bool drain_pass_warm(const SpDev& T, SM& sm, ReqState& rs, bool final
   return HF && hf_capped && !rs.deferred;
 }
 
-template <bool SMALL, bool LONG, int MODE, bool MEMO, bool WARM = false, typename SM>
+template <bool SMALL, bool LONG, int MODE, bool MEMO, bool WARM, typename SM>
 __device__ __forceinline__ void drain(const SpDev& T, SM& sm, ReqState& rs, bool final, int lane, MemoRef memo) {
-  if constexpr (WARM) {
-    if constexpr (MODE == 1) {
-      while (drain_pass_warm<SMALL, LONG, 1, MEMO>(T, sm, rs, final, lane, memo)) {}
-    } else {
-      drain_pass_warm<SMALL, LONG, MODE, MEMO>(T, sm, rs, final, lane, memo);
-    }
-  } else if constexpr (MODE == 1) {
-    while (drain_pass<SMALL, LONG, 1, MEMO>(T, sm, rs, final, lane, memo)) {}
+  if constexpr (MODE == 1) {
+    while (drain_pass<SMALL, LONG, 1, MEMO, WARM>(T, sm, rs, final, lane, memo)) {}
   } else {
-    drain_pass<SMALL, LONG, MODE, MEMO>(T, sm, rs, final, lane, memo);
+    drain_pass<SMALL, LONG, MODE, MEMO, WARM>(T, sm, rs, final, lane, memo);
   }
 }
 
@@ -2676,7 +2262,7 @@ __device__ __forceinline__ void drain(const SpDev& T, SM& sm, ReqState& rs, bool
 // LONG == true : re-runs exactly the deferred requests (work list = defer_list[0 .. *defer_count)).
 // HF == true : byte-level BPE with the regex pre-tokenizer (split_mode 3).
 // MEMO == true: words are looked up in / added to the launch's word memo (never built together with LONG).
-// WARM == true: drains go through drain_pass_warm (natural text; MEMO kernels only).
+// WARM == true: drains run the warm-up pre-passes of drain_pass (natural text; MEMO kernels only).
 template <bool SMALL, bool LONG, int MODE, bool MEMO, bool WARM = false>
 __global__ void __launch_bounds__(32, LONG ? 8 : ((MODE != 2 && !WARM) ? 16 : 27)) sp_encode_kernel(
     const uint8_t* __restrict__ text, const int64_t* __restrict__ offsets, int n_req, int32_t* __restrict__ ids,
@@ -3035,12 +2621,10 @@ int SpDeviceModel::upload(const SpTables& t) {
 
 static DeviceOnce g_sp_once;
 
-static int sp_warps_per_sm(const SpDev& dev, bool warm = false) {
-  const bool small = dev.small_vocab != 0;
-  const bool hf = !warm;   // every buffer-path BPE kernel has 32-row columns; the warm-up kernels keep 16
-  const size_t smem = dev.unigram ? (small ? sizeof(WarpSmemUniT<true>) : sizeof(WarpSmemUniT<false>))
-                      : hf        ? (small ? sizeof(WarpSmemT<true, kHfRows>) : sizeof(WarpSmemT<false, kHfRows>))
-                                  : (small ? sizeof(WarpSmemT<true>) : sizeof(WarpSmemT<false>));
+// Resident one-warp blocks per SM of a buffer-path kernel whose warp takes smem bytes of shared memory: as many as
+// 227 KB holds with 1 KB reserved per block, at most 27.  XLLM_SP_WARPS_PER_SM may lower it, except for Unigram.
+// The warm-up arena (sp_warm_arena_bytes) and the warm launch's grid are both sized from it.
+static int sp_warps_per_sm(const SpDev& dev, size_t smem) {
   int w = (int)((227 * 1024) / (smem + 1024));
   if (w > 27) w = 27;
   if (!dev.unigram && g_warps_per_sm_override > 0 && g_warps_per_sm_override < w) w = g_warps_per_sm_override;
@@ -3051,7 +2635,12 @@ static int sp_legacy_grid(const SpDev& dev, int n_req, bool warm = false) {
   int n_sm = 0, d = 0;
   if (cudaGetDevice(&d) != cudaSuccess || cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, d) != cudaSuccess)
     return 0;
-  const int grid = n_sm * sp_warps_per_sm(dev, warm);
+  const bool small = dev.small_vocab != 0;
+  const bool hf = !warm;   // every buffer-path BPE kernel has 32-row columns; the warm-up kernels keep 16
+  const size_t smem = dev.unigram ? (small ? sizeof(WarpSmemUniT<true>) : sizeof(WarpSmemUniT<false>))
+                      : hf        ? (small ? sizeof(WarpSmemT<true, kHfRows>) : sizeof(WarpSmemT<false, kHfRows>))
+                                  : (small ? sizeof(WarpSmemT<true>) : sizeof(WarpSmemT<false>));
+  const int grid = n_sm * sp_warps_per_sm(dev, smem);
   return grid > n_req ? n_req : grid;
 }
 size_t sp_warm_arena_bytes(const SpDev& dev, int n_req) { return (size_t)sp_legacy_grid(dev, n_req, true) * kWarmSliceBytes; }
@@ -3165,10 +2754,7 @@ cudaError_t sp_encode_launch(const SpDev& dev_in, const uint8_t* text, const int
   cudaError_t e = cudaMemsetAsync(counters, 0, 5 * sizeof(unsigned int), stream);
   if (e != cudaSuccess) return e;
   auto grid_for = [&](size_t smem_bytes) {
-    int warps_per_sm = (int)((227 * 1024) / (smem_bytes + 1024));
-    if (warps_per_sm > 27) warps_per_sm = 27;
-    if (g_warps_per_sm_override > 0 && g_warps_per_sm_override < warps_per_sm) warps_per_sm = g_warps_per_sm_override;
-    const int g = n_sm * warps_per_sm;
+    const int g = n_sm * sp_warps_per_sm(dev, smem_bytes);
     return g > n_req ? n_req : g;
   };
   int grid_long = n_sm * 2;
@@ -3178,7 +2764,7 @@ cudaError_t sp_encode_launch(const SpDev& dev_in, const uint8_t* text, const int
     e = cudaMemsetAsync(memo.table, 0, (size_t)memo.slots * 32, stream);  // default policy: the memo lives for this launch only
     if (e != cudaSuccess) return e;
   }
-  // the warm-up kernels (drain_pass_warm) need their per-warp scratch; the caller passes it only when they are wanted
+  // the warm-up kernels (drain_pass<..., WARM>) need their per-warp scratch; the caller passes it only when they are wanted
   const bool warm = use_memo && !dev.unigram && memo.arena != nullptr &&
                     memo.arena_bytes >= (size_t)grid_for(smem16) * kWarmSliceBytes;
   const size_t smem = warm ? smem16 : smem_long;   // the throughput kernel's shared memory: 16-row columns when warm
@@ -3213,10 +2799,7 @@ cudaError_t sp_encode_launch(const SpDev& dev_in, const uint8_t* text, const int
   if (dev.unigram) {
     // Viterbi per word from a running score: no word memo (the result depends on the prefix), no long-word pass
     const size_t usmem = small ? sizeof(WarpSmemUniT<true>) : sizeof(WarpSmemUniT<false>);
-    int uwarps = (int)((227 * 1024) / (usmem + 1024));
-    if (uwarps > 27) uwarps = 27;
-    int ugrid = n_sm * uwarps;
-    if (ugrid > n_req) ugrid = n_req;
+    const int ugrid = grid_for(usmem);
     if (small)
       sp_encode_kernel<true, false, 2, false><<<ugrid, 32, usmem, stream>>>(
           text, offsets, n_req, ids, ids_stride, n_ids, status, dev, counters, defer_list, counters + 1, nullptr, 0u);

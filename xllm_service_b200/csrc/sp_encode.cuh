@@ -66,7 +66,7 @@ struct SpDev {
   const int64_t* out_start;      // request r's ids go to ids + out_start[r] (at most out_cap[r]) instead of r * ids_stride
   const int32_t* out_cap;
   unsigned long long* warp_ns;   // [grid]: nanoseconds each warp of the throughput kernel spent from start to exit
-  uint8_t* warm_arena;           // [grid] slices of sp_warm_slice_bytes(): scratch of the warm-up pre-passes (sp_encode.cu 1b)
+  uint8_t* warm_arena;           // [grid] slices of kWarmSliceBytes: scratch of the warm-up pre-passes (sp_encode.cu drain_pass 1b)
   const int32_t* work_list;      // buffer-path kernel after the express kernel: the requests handed over, their count,
   const unsigned int* work_count;  // and where each one resumes (ExpResume records, sp_encode.cu)
   const void* resume;
