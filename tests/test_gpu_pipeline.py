@@ -161,3 +161,11 @@ def test_narrow_id_download_equals_int32(oracle):
         hw.close()
     finally:
         del os.environ["XLLM_SP_FORCE_WIDE"]
+    # 128 471 entries: ids past 65 535 cannot be downloaded as uint16
+    hb = x.Ingest(tokenizer_path=os.path.join(HERE, "golden", "hf_natural_128k"))
+    try:
+        with pytest.raises(x.IngestError) as e:
+            hb.ingest_batch(b.text, b.offsets, 200, want_match=False, ids_u16=True)
+        assert e.value.code == -5      # XLLM_ERR_UNSUPPORTED
+    finally:
+        hb.close()
