@@ -184,6 +184,10 @@ typedef struct {
 
 /* keys: the block keys of all requests; request r owns n_blocks[r] keys starting at key_start[r].
  * match / routing may be NULL.  Host-pointer and device-pointer forms.
+ * n_blocks[r] must be at most 65 535 (the scores are 16-bit).  xllm_match_route checks it and fails with
+ * XLLM_ERR_INVALID_ARG; xllm_match_route_device and xllm_score_route_device read n_blocks on the device and cannot
+ * check it without a synchronisation, so there the limit is the caller's to keep.
+ * The device-pointer calls of one handle share its counters and scratch: issue them in order on one stream.
  * With a sharded index these two calls and xllm_ingest_batch (when match / routing is requested) are COLLECTIVE: every
  * rank must make the call once per batch (each with its own requests, n_req may be 0); they synchronise the stream. */
 int xllm_match_route(xllm_ingest_t h, int32_t n_req, const uint8_t* keys, int64_t n_keys_total,
@@ -237,7 +241,12 @@ int xllm_encode_batch_device(xllm_ingest_t h, int32_t n_req, const uint8_t* d_te
  * pipelined in chunks over several CUDA streams; pass page-locked buffers (xllm_host_alloc) so
  * the PCIe copies overlap the kernels.  keys / match / routing may be NULL to skip those outputs
  * (match or routing != NULL requires an index).  keys_stride = 16-byte keys per request row
- * (0 => ids_stride / block_size); rows are zero-padded past floor(n_ids/block_size).
+ * (0 => ids_stride / block_size); rows are zero-padded past floor(n_ids/block_size).  keys_stride also caps the
+ * blocks that are hashed and matched: a row's keys, match and routing cover its first
+ * min(keys_stride, floor(min(n_ids, ids_stride)/block_size)) blocks.
+ * Match scores are 16-bit (xllm_match_out): with match or routing requested, a batch whose rows can hold more than
+ * 65 535 blocks (min(keys_stride, ids_stride / block_size) > 65 535) is refused with XLLM_ERR_INVALID_ARG before any
+ * work is queued.  Keys alone have no such limit.
  */
 typedef struct {
   int32_t n_req;

@@ -252,6 +252,15 @@ static int ingest_core(xllm_ingest_t h, const xllm_ingest_io* io, const xllm_seg
     return XLLM_ERR_UNSUPPORTED;
   }
   const int64_t keys_stride = io->keys_stride > 0 ? io->keys_stride : (want_match ? io->ids_stride / h->block_size : 0);
+  // xllm_match_out keeps scores as uint16 (1 + the last matched block index, shard tuples carry the block index in 16
+  // bits too): a row of more than 65 535 blocks would wrap and report an instance holding every block as absent
+  const int64_t max_row_blocks = std::min(keys_stride, io->ids_stride / h->block_size);
+  if (want_match && max_row_blocks > 65535) {
+    set_last_error("xllm_ingest_batch: match / routing of rows of up to %lld blocks requested, the limit is 65535 "
+                   "(ids_stride %lld, keys_stride %lld, block_size %d)", (long long)max_row_blocks,
+                   (long long)io->ids_stride, (long long)io->keys_stride, h->block_size);
+    return XLLM_ERR_INVALID_ARG;
+  }
   // ---- segmented requests: where each request's text pieces and id spans start (host prefix sums)
   int64_t n_pieces = n;                    // rows of io->offsets: requests, or text pieces
   std::vector<int64_t> piece_of_req, span_of_req, seg_src;   // [n + 1], [n + 1], [n_segments]
