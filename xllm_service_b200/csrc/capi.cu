@@ -59,15 +59,29 @@ void PinBuf::release() {
   cap = 0;
 }
 
+int encode_reserve(xllm_ingest* h, int n_req, DevBuf* scratch, DevBuf* memo_buf, int64_t* memo_age, SpMemo* memo,
+                   SpEncodePlan* plan) {
+  XLLM_CUDA_TRY(sp_encode_plan(h->sp_dev->dev(), n_req, h->memo_slots != 0, h->sp_warm, plan));
+  XLLM_TRY_RC(scratch->reserve(plan->scratch_bytes));
+  *memo = SpMemo();
+  if (plan->memo) {
+    XLLM_TRY_RC(memo_buf->reserve((size_t)h->memo_slots * 32));
+    memo->table = memo_buf->p;
+    memo->slots = h->memo_slots;
+    memo->clear = memo_needs_clear(h->memo_persist_requests, memo_age, n_req);
+  }
+  if (plan->warm) {   // one arena per handle: its launches, pipeline chunks included, run one after the other
+    XLLM_TRY_RC(h->d_arena.reserve(plan->arena_bytes));   // the full grid's worth: never regrown
+    memo->warm = true;
+    memo->arena = h->d_arena.p;
+    memo->arena_bytes = plan->arena_bytes;
+  }
+  return XLLM_OK;
+}
+
 }  // namespace xllm
 
 using namespace xllm;
-
-#define XLLM_TRY(expr)          \
-  do {                          \
-    int _rc = (expr);           \
-    if (_rc != XLLM_OK) return _rc; \
-  } while (0)
 
 extern "C" {
 
@@ -279,11 +293,11 @@ int xllm_hash_blocks(xllm_ingest_t h, int32_t n_req, const int32_t* tokens, int6
   }
   std::lock_guard<std::mutex> lock(h->mu);
   XLLM_CUDA_TRY(cudaSetDevice(h->device));
-  XLLM_TRY(h->d_tokens.reserve((size_t)n_tokens_total * 4 + 16));
-  XLLM_TRY(h->d_tok_start.reserve((size_t)n_req * 8));
-  XLLM_TRY(h->d_n_tok.reserve((size_t)n_req * 4));
-  XLLM_TRY(h->d_keys.reserve((size_t)n_keys_total * 16 + 16));
-  XLLM_TRY(h->d_key_start.reserve((size_t)n_req * 8));
+  XLLM_TRY_RC(h->d_tokens.reserve((size_t)n_tokens_total * 4 + 16));
+  XLLM_TRY_RC(h->d_tok_start.reserve((size_t)n_req * 8));
+  XLLM_TRY_RC(h->d_n_tok.reserve((size_t)n_req * 4));
+  XLLM_TRY_RC(h->d_keys.reserve((size_t)n_keys_total * 16 + 16));
+  XLLM_TRY_RC(h->d_key_start.reserve((size_t)n_req * 8));
   cudaStream_t s = h->stream;
   XLLM_CUDA_TRY(cudaMemcpyAsync(h->d_tokens.p, tokens, (size_t)n_tokens_total * 4, cudaMemcpyHostToDevice, s));
   XLLM_CUDA_TRY(cudaMemcpyAsync(h->d_tok_start.p, tok_start, (size_t)n_req * 8, cudaMemcpyHostToDevice, s));
@@ -314,8 +328,8 @@ int xllm_xxh3_128bits_hash(xllm_ingest_t h, const uint8_t* prev16, const int32_t
   std::lock_guard<std::mutex> lock(h->mu);
   XLLM_CUDA_TRY(cudaSetDevice(h->device));
   const size_t n = n_tokens + (prev16 ? 4 : 0);
-  XLLM_TRY(h->d_tokens.reserve(n * 4 + 16));
-  XLLM_TRY(h->d_keys.reserve(32));
+  XLLM_TRY_RC(h->d_tokens.reserve(n * 4 + 16));
+  XLLM_TRY_RC(h->d_keys.reserve(32));
   cudaStream_t s = h->stream;
   uint8_t* dt = h->d_tokens.as<uint8_t>();
   if (prev16) XLLM_CUDA_TRY(cudaMemcpyAsync(dt, prev16, 16, cudaMemcpyHostToDevice, s));
@@ -376,7 +390,7 @@ static int need_index(xllm_ingest_t h) {
 
 int xllm_index_apply(xllm_ingest_t h, int32_t instance_id, const uint8_t* stored, size_t n_stored,
                      const uint8_t* offload, size_t n_offload, const uint8_t* removed, size_t n_removed) {
-  XLLM_TRY(need_index(h));
+  XLLM_TRY_RC(need_index(h));
   if (instance_id < 0 || instance_id >= kMaxInstances || (n_stored && !stored) || (n_offload && !offload) ||
       (n_removed && !removed)) {
     set_last_error("xllm_index_apply: invalid argument");
@@ -398,7 +412,7 @@ int xllm_index_apply(xllm_ingest_t h, int32_t instance_id, const uint8_t* stored
   return XLLM_OK;
 }
 int xllm_index_put(xllm_ingest_t h, const uint8_t* key16, uint64_t hbm, uint64_t dram, uint64_t ssd) {
-  XLLM_TRY(need_index(h));
+  XLLM_TRY_RC(need_index(h));
   if (!key16) return XLLM_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(*h->index_mu);
   if (!owns_key(h, key16)) return XLLM_OK;
@@ -407,7 +421,7 @@ int xllm_index_put(xllm_ingest_t h, const uint8_t* key16, uint64_t hbm, uint64_t
 }
 int xllm_index_put_bulk(xllm_ingest_t h, int64_t n, const uint8_t* keys, const uint64_t* hbm, const uint64_t* dram,
                         const uint64_t* ssd) {
-  XLLM_TRY(need_index(h));
+  XLLM_TRY_RC(need_index(h));
   if (n < 0 || (n > 0 && (!keys || !hbm || !dram || !ssd))) return XLLM_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(*h->index_mu);
   for (int64_t i = 0; i < n; ++i)
@@ -416,7 +430,7 @@ int xllm_index_put_bulk(xllm_ingest_t h, int64_t n, const uint8_t* keys, const u
 }
 int xllm_index_export(xllm_ingest_t h, int64_t capacity, uint8_t* keys, uint64_t* hbm, uint64_t* dram, uint64_t* ssd,
                       int64_t* n_keys) {
-  XLLM_TRY(need_index(h));
+  XLLM_TRY_RC(need_index(h));
   if (!n_keys || capacity < 0 || (capacity > 0 && (!keys || !hbm || !dram || !ssd))) return XLLM_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(h->mu);
   std::lock_guard<std::mutex> lock2(*h->index_mu);
@@ -424,7 +438,7 @@ int xllm_index_export(xllm_ingest_t h, int64_t capacity, uint8_t* keys, uint64_t
   return h->index->export_all(h->stream, capacity, keys, hbm, dram, ssd, n_keys);
 }
 int xllm_index_erase(xllm_ingest_t h, const uint8_t* key16) {
-  XLLM_TRY(need_index(h));
+  XLLM_TRY_RC(need_index(h));
   if (!key16) return XLLM_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(*h->index_mu);
   if (!owns_key(h, key16)) return XLLM_OK;
@@ -432,14 +446,14 @@ int xllm_index_erase(xllm_ingest_t h, const uint8_t* key16) {
   return XLLM_OK;
 }
 int xllm_index_publish(xllm_ingest_t h) {
-  XLLM_TRY(need_index(h));
+  XLLM_TRY_RC(need_index(h));
   std::lock_guard<std::mutex> lock(h->mu);
   std::lock_guard<std::mutex> lock2(*h->index_mu);
   XLLM_CUDA_TRY(cudaSetDevice(h->device));
   return h->index->publish(h->stream);
 }
 int xllm_index_clear_instance(xllm_ingest_t h, int32_t instance_id) {
-  XLLM_TRY(need_index(h));
+  XLLM_TRY_RC(need_index(h));
   if (instance_id < 0 || instance_id >= kMaxInstances) {
     set_last_error("xllm_index_clear_instance: invalid instance id %d", instance_id);
     return XLLM_ERR_INVALID_ARG;
@@ -450,7 +464,7 @@ int xllm_index_clear_instance(xllm_ingest_t h, int32_t instance_id) {
   return h->index->clear_instance(h->stream, instance_id);
 }
 int xllm_index_stats(xllm_ingest_t h, int64_t* live_keys, int64_t* tombstones, int64_t* rebuilds) {
-  XLLM_TRY(need_index(h));
+  XLLM_TRY_RC(need_index(h));
   std::lock_guard<std::mutex> lock2(*h->index_mu);
   if (live_keys) *live_keys = h->index->live_keys();
   if (tombstones) *tombstones = h->index->tombstones();
@@ -458,14 +472,14 @@ int xllm_index_stats(xllm_ingest_t h, int64_t* live_keys, int64_t* tombstones, i
   return XLLM_OK;
 }
 int xllm_index_size(xllm_ingest_t h, int64_t* n_keys) {
-  XLLM_TRY(need_index(h));
+  XLLM_TRY_RC(need_index(h));
   if (!n_keys) return XLLM_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(h->mu);
   XLLM_CUDA_TRY(cudaSetDevice(h->device));
   return h->index->size(h->stream, n_keys);
 }
 int xllm_index_get(xllm_ingest_t h, const uint8_t* key16, uint64_t masks3[3], int32_t* found) {
-  XLLM_TRY(need_index(h));
+  XLLM_TRY_RC(need_index(h));
   if (!key16 || !masks3 || !found) return XLLM_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(h->mu);
   std::lock_guard<std::mutex> lock2(*h->index_mu);
@@ -514,7 +528,7 @@ static int sync_instances(xllm_ingest_t h, cudaStream_t s) {
 
 int xllm_index_probe_device(xllm_ingest_t h, const uint8_t* d_keys, int64_t n_keys, uint64_t* d_masks3,
                             void* cuda_stream) {
-  XLLM_TRY(need_index(h));
+  XLLM_TRY_RC(need_index(h));
   if (n_keys < 0 || (n_keys > 0 && (!d_keys || !d_masks3))) return XLLM_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(h->mu);
   XLLM_CUDA_TRY(cudaSetDevice(h->device));
@@ -533,7 +547,7 @@ int xllm_score_route_device(xllm_ingest_t h, int32_t n_req, const uint64_t* d_ma
   std::lock_guard<std::mutex> lock(h->mu);
   XLLM_CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : h->stream;
-  XLLM_TRY(sync_instances(h, s));
+  XLLM_TRY_RC(sync_instances(h, s));
   XLLM_CUDA_TRY(score_route_launch(d_masks3, d_key_start, d_n_blocks, n_req, h->d_inst,
                                    reinterpret_cast<MatchOut*>(d_match), reinterpret_cast<RoutingOut*>(d_routing), s));
   return XLLM_OK;
@@ -542,14 +556,14 @@ int xllm_score_route_device(xllm_ingest_t h, int32_t n_req, const uint64_t* d_ma
 int xllm_match_route_device(xllm_ingest_t h, int32_t n_req, const uint8_t* d_keys, int64_t n_keys_total,
                             const int64_t* d_key_start, const int32_t* d_n_blocks, xllm_match_out* d_match,
                             xllm_routing_out* d_routing, void* cuda_stream) {
-  XLLM_TRY(need_index(h));
+  XLLM_TRY_RC(need_index(h));
   if (n_req < 0 || n_keys_total < 0 || (n_req > 0 && (!d_key_start || !d_n_blocks)) || (n_keys_total > 0 && !d_keys))
     return XLLM_ERR_INVALID_ARG;
   if (n_req == 0 && !h->shard) return XLLM_OK;   // a sharded round is collective: an empty rank still takes part
   std::lock_guard<std::mutex> lock(h->mu);
   XLLM_CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : h->stream;
-  XLLM_TRY(sync_instances(h, s));   // takes index_mu: before begin_read, never inside (publish: index_mu -> writer lock)
+  XLLM_TRY_RC(sync_instances(h, s));   // takes index_mu: before begin_read, never inside (publish: index_mu -> writer lock)
   if (h->shard)   // collective; synchronises `s`
     return h->shard->match_route(*h->index, h->index_read_ev, d_keys, d_key_start, d_n_blocks, n_req, n_keys_total,
                                  h->d_inst, reinterpret_cast<MatchOut*>(d_match),
@@ -566,7 +580,7 @@ int xllm_match_route_device(xllm_ingest_t h, int32_t n_req, const uint8_t* d_key
 int xllm_match_route(xllm_ingest_t h, int32_t n_req, const uint8_t* keys, int64_t n_keys_total,
                      const int64_t* key_start, const int32_t* n_blocks, xllm_match_out* match,
                      xllm_routing_out* routing) {
-  XLLM_TRY(need_index(h));
+  XLLM_TRY_RC(need_index(h));
   if (n_req < 0 || n_keys_total < 0 || (n_req > 0 && (!key_start || !n_blocks)) || (n_keys_total > 0 && !keys))
     return XLLM_ERR_INVALID_ARG;
   if (n_req == 0 && !h->shard) return XLLM_OK;   // a sharded round is collective: an empty rank still takes part
@@ -578,20 +592,20 @@ int xllm_match_route(xllm_ingest_t h, int32_t n_req, const uint8_t* keys, int64_
   std::lock_guard<std::mutex> lock(h->mu);
   XLLM_CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = h->stream;
-  XLLM_TRY(h->d_keys.reserve((size_t)n_keys_total * 16 + 64));
-  XLLM_TRY(h->d_key_start.reserve((size_t)n_req * 8 + 8));
-  XLLM_TRY(h->d_nblk.reserve((size_t)n_req * 4 + 8));
-  XLLM_TRY(h->d_match.reserve((size_t)n_req * sizeof(MatchOut) + 8));
-  XLLM_TRY(h->d_routing.reserve((size_t)n_req * sizeof(RoutingOut) + 8));
+  XLLM_TRY_RC(h->d_keys.reserve((size_t)n_keys_total * 16 + 64));
+  XLLM_TRY_RC(h->d_key_start.reserve((size_t)n_req * 8 + 8));
+  XLLM_TRY_RC(h->d_nblk.reserve((size_t)n_req * 4 + 8));
+  XLLM_TRY_RC(h->d_match.reserve((size_t)n_req * sizeof(MatchOut) + 8));
+  XLLM_TRY_RC(h->d_routing.reserve((size_t)n_req * sizeof(RoutingOut) + 8));
   if (n_keys_total)
     XLLM_CUDA_TRY(cudaMemcpyAsync(h->d_keys.p, keys, (size_t)n_keys_total * 16, cudaMemcpyHostToDevice, s));
   if (n_req) {
     XLLM_CUDA_TRY(cudaMemcpyAsync(h->d_key_start.p, key_start, (size_t)n_req * 8, cudaMemcpyHostToDevice, s));
     XLLM_CUDA_TRY(cudaMemcpyAsync(h->d_nblk.p, n_blocks, (size_t)n_req * 4, cudaMemcpyHostToDevice, s));
   }
-  XLLM_TRY(sync_instances(h, s));
+  XLLM_TRY_RC(sync_instances(h, s));
   if (h->shard) {
-    XLLM_TRY(h->shard->match_route(*h->index, h->index_read_ev, h->d_keys.as<uint8_t>(), h->d_key_start.as<int64_t>(),
+    XLLM_TRY_RC(h->shard->match_route(*h->index, h->index_read_ev, h->d_keys.as<uint8_t>(), h->d_key_start.as<int64_t>(),
                                    h->d_nblk.as<int32_t>(), n_req, n_keys_total, h->d_inst, h->d_match.as<MatchOut>(),
                                    h->d_routing.as<RoutingOut>(), s));
   } else {
@@ -679,19 +693,9 @@ int xllm_encode_batch_device(xllm_ingest_t h, int32_t n_req, const uint8_t* d_te
   std::lock_guard<std::mutex> lock(h->mu);
   XLLM_CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : h->stream;
-  XLLM_TRY(h->d_defer.reserve(xllm::sp_encode_scratch_bytes(n_req)));
   SpMemo memo;
-  if (h->memo_slots) {
-    XLLM_TRY(h->d_memo.reserve((size_t)h->memo_slots * 32));
-    memo.table = h->d_memo.p;
-    memo.slots = h->memo_slots;
-    memo.clear = xllm::memo_needs_clear(h->memo_persist_requests, &h->memo_age, n_req);
-    if (h->sp_warm) {
-      memo.arena_bytes = sp_warm_arena_bytes(h->sp_dev->dev(), 1 << 30);   // the full grid's worth: never regrown
-      XLLM_TRY(h->d_arena.reserve(memo.arena_bytes));
-      memo.arena = h->d_arena.p;
-    }
-  }
+  SpEncodePlan plan;
+  XLLM_TRY_RC(encode_reserve(h, n_req, &h->d_defer, &h->d_memo, &h->memo_age, &memo, &plan));
   XLLM_CUDA_TRY(sp_encode_launch(h->sp_dev->dev(), d_text, d_offsets, n_req, d_ids, ids_stride, d_n_ids, d_status,
                                  h->d_task_counter + 4, h->d_defer.p, s, memo));
   return XLLM_OK;
@@ -720,34 +724,23 @@ static int encode_batch_impl(xllm_ingest_t h, int32_t n_req, const uint8_t* text
   if (text_bytes > 0 && !text) return XLLM_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(h->mu);
   XLLM_CUDA_TRY(cudaSetDevice(h->device));
-  XLLM_TRY(h->d_text.reserve(text_bytes + 16));
-  XLLM_TRY(h->d_offsets.reserve((size_t)(n_req + 1) * 8));
-  XLLM_TRY(h->d_ids.reserve((size_t)n_req * (size_t)ids_stride * 4 + 16));
-  XLLM_TRY(h->d_n_ids.reserve((size_t)n_req * 4));
-  XLLM_TRY(h->d_status.reserve((size_t)n_req * 4));
-  XLLM_TRY(h->d_defer.reserve(xllm::sp_encode_scratch_bytes(n_req)));
+  XLLM_TRY_RC(h->d_text.reserve(text_bytes + 16));
+  XLLM_TRY_RC(h->d_offsets.reserve((size_t)(n_req + 1) * 8));
+  XLLM_TRY_RC(h->d_ids.reserve((size_t)n_req * (size_t)ids_stride * 4 + 16));
+  XLLM_TRY_RC(h->d_n_ids.reserve((size_t)n_req * 4));
+  XLLM_TRY_RC(h->d_status.reserve((size_t)n_req * 4));
   cudaStream_t s = h->stream;
   SpMemo memo;
-  if (h->memo_slots) {
-    XLLM_TRY(h->d_memo.reserve((size_t)h->memo_slots * 32));
-    memo.table = h->d_memo.p;
-    memo.slots = h->memo_slots;
-    memo.clear = xllm::memo_needs_clear(h->memo_persist_requests, &h->memo_age, n_req);
-    if (h->sp_warm) {
-      memo.arena_bytes = sp_warm_arena_bytes(h->sp_dev->dev(), 1 << 30);   // the full grid's worth: never regrown
-      XLLM_TRY(h->d_arena.reserve(memo.arena_bytes));
-      memo.arena = h->d_arena.p;
-    }
-  }
+  SpEncodePlan plan;
+  XLLM_TRY_RC(encode_reserve(h, n_req, &h->d_defer, &h->d_memo, &h->memo_age, &memo, &plan));
   // offsets are rebased on the device copy of the text: ship them relative to offsets[0]
   if (text_bytes)
     XLLM_CUDA_TRY(cudaMemcpyAsync(h->d_text.p, text + offsets[0], text_bytes, cudaMemcpyHostToDevice, s));
   XLLM_CUDA_TRY(cudaMemcpyAsync(h->d_offsets.p, offsets, (size_t)(n_req + 1) * 8, cudaMemcpyHostToDevice, s));
   SpLaunchOpts opts;
-  int grid = 0;
+  const int grid = plan.warp_ns;
   if (warp_ns) {   // diagnostics: per-warp busy time of the persistent grid
-    grid = sp_encode_grid(h->sp_dev->dev(), n_req);
-    XLLM_TRY(h->d_masks.reserve((size_t)grid * 8 + 8));
+    XLLM_TRY_RC(h->d_masks.reserve((size_t)grid * 8 + 8));
     XLLM_CUDA_TRY(cudaMemsetAsync(h->d_masks.p, 0, (size_t)grid * 8, s));
     opts.warp_ns = h->d_masks.as<unsigned long long>();
   }

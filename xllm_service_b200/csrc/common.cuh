@@ -60,12 +60,14 @@ struct DeviceOnce {
   std::once_flag flag[kMaxDevices];
   int n_sm[kMaxDevices] = {0};
   cudaError_t err[kMaxDevices] = {cudaSuccess};
-  // runs setup(dev) exactly once per device; returns that device's SM count (0 on error, *e set)
+  // runs setup() exactly once per device; returns that device's SM count (0 on error, *e set).  *device, if given, is
+  // set to the current device before setup runs.
   template <typename F>
-  int get(F&& setup, cudaError_t* e) {
+  int get(F&& setup, cudaError_t* e, int* device = nullptr) {
     int dev = 0;
     *e = cudaGetDevice(&dev);
     if (*e != cudaSuccess) return 0;
+    if (device) *device = dev;
     if (dev < 0 || dev >= kMaxDevices) { *e = cudaErrorInvalidDevice; return 0; }
     std::call_once(flag[dev], [&] {
       int n = 0;

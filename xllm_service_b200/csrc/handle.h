@@ -104,3 +104,11 @@ struct xllm_ingest {
   // sharded xllm_ingest_batch: the whole batch's keys / row descriptors / results stay resident for the one exchange
   xllm::DevBuf d_all_keys, d_all_key_start, d_all_n_blocks, d_all_match, d_all_routing;
 };
+
+namespace xllm {
+// Plans one sp_encode_launch over n_req rows on handle h and reserves what it needs: the launch scratch, the word memo
+// table and the warm-up arena.  memo_buf / memo_age: the handle's or the pipeline slot's table and its age
+// (xllm_set_memo_policy), which this launch advances.  Fills *memo for the launch.
+int encode_reserve(xllm_ingest* h, int n_req, DevBuf* scratch, DevBuf* memo_buf, int64_t* memo_age, SpMemo* memo,
+                   SpEncodePlan* plan);
+}  // namespace xllm

@@ -123,7 +123,6 @@ int PipeSlot::ensure(size_t text_bytes, int n, int64_t ids_stride, int64_t keys_
   if ((rc = d_ids.reserve((size_t)n_req * (size_t)ids_stride * 4 + 64)) != XLLM_OK) return rc;
   if ((rc = d_n_ids.reserve((size_t)n * 4)) != XLLM_OK) return rc;
   if ((rc = d_status.reserve((size_t)n * 4)) != XLLM_OK) return rc;
-  if ((rc = d_defer.reserve(xllm::sp_encode_scratch_bytes(n))) != XLLM_OK) return rc;
   if ((rc = d_tok_start.reserve((size_t)n * 8)) != XLLM_OK) return rc;
   if ((rc = d_n_tok.reserve((size_t)n * 4)) != XLLM_OK) return rc;
   if ((rc = d_key_start.reserve((size_t)n * 8)) != XLLM_OK) return rc;
@@ -155,12 +154,6 @@ void PipeSlot::release() {
 }  // namespace xllm
 
 using namespace xllm;
-
-#define XLLM_TRY(expr)              \
-  do {                              \
-    int _rc = (expr);               \
-    if (_rc != XLLM_OK) return _rc; \
-  } while (0)
 
 extern "C" {
 
@@ -312,11 +305,11 @@ static int ingest_core(xllm_ingest_t h, const xllm_ingest_io* io, const xllm_seg
   // for the whole batch follows the last chunk (collective: every rank makes this call once per batch)
   const bool sharded = want_match && h->shard != nullptr;
   if (sharded) {
-    XLLM_TRY(h->d_all_keys.reserve((size_t)n * (size_t)keys_stride * 16 + 64));
-    XLLM_TRY(h->d_all_key_start.reserve((size_t)n * 8));
-    XLLM_TRY(h->d_all_n_blocks.reserve((size_t)n * 4));
-    XLLM_TRY(h->d_all_match.reserve((size_t)n * sizeof(MatchOut)));
-    XLLM_TRY(h->d_all_routing.reserve((size_t)n * sizeof(RoutingOut)));
+    XLLM_TRY_RC(h->d_all_keys.reserve((size_t)n * (size_t)keys_stride * 16 + 64));
+    XLLM_TRY_RC(h->d_all_key_start.reserve((size_t)n * 8));
+    XLLM_TRY_RC(h->d_all_n_blocks.reserve((size_t)n * 4));
+    XLLM_TRY_RC(h->d_all_match.reserve((size_t)n * sizeof(MatchOut)));
+    XLLM_TRY_RC(h->d_all_routing.reserve((size_t)n * sizeof(RoutingOut)));
   }
   if (want_match) {
     std::lock_guard<std::mutex> l2(*h->index_mu);
@@ -386,16 +379,9 @@ static int ingest_core(xllm_ingest_t h, const xllm_ingest_io* io, const xllm_seg
     // the slot's previous chunk has been downloaded (host wait: ensure() below may reallocate its buffers)
     if (sl.busy) PIPE_CUDA_TRY(cudaEventSynchronize(sl.ev[2]));
     if ((rc = sl.ensure(text_bytes, m > mp ? m : mp, io->ids_stride, keys_stride, m)) != XLLM_OK) break;
-    if (h->memo_slots && (rc = sl.d_memo.reserve((size_t)h->memo_slots * 32)) != XLLM_OK) break;
     xllm::SpMemo memo;
-    memo.table = h->memo_slots ? sl.d_memo.p : nullptr;
-    memo.slots = h->memo_slots;
-    if (h->memo_slots) memo.clear = xllm::memo_needs_clear(h->memo_persist_requests, &sl.memo_age, seg ? (int64_t)(p1 - p0) : (int64_t)m);
-    if (h->memo_slots && h->sp_warm) {   // kernels of all chunks run on one stream, one after the other: one scratch for the handle
-      memo.arena_bytes = sp_warm_arena_bytes(h->sp_dev->dev(), 1 << 30);   // the full grid's worth: never regrown
-      if ((rc = h->d_arena.reserve(memo.arena_bytes)) != XLLM_OK) break;
-      memo.arena = h->d_arena.p;
-    }
+    xllm::SpEncodePlan plan;
+    if ((rc = encode_reserve(h, mp, &sl.d_defer, &sl.d_memo, &sl.memo_age, &memo, &plan)) != XLLM_OK) break;
     if (trace) {
       rows.push_back(TraceRow{m, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count(), {}});
       mark(0, s_in);
@@ -434,7 +420,6 @@ static int ingest_core(xllm_ingest_t h, const xllm_ingest_io* io, const xllm_seg
       if ((rc = sl.d_seg_src.reserve((size_t)(s1 - s0) * 8 + 8)) != XLLM_OK) break;
       if ((rc = sl.d_req_seg.reserve((size_t)(m + 1) * 4)) != XLLM_OK) break;
       if ((rc = sl.d_span.reserve((size_t)(sp1 - sp0) * 4 + 4)) != XLLM_OK) break;
-      if ((rc = sl.d_defer.reserve(xllm::sp_encode_scratch_bytes(mp))) != XLLM_OK) break;
       if (mp) {
         PIPE_CUDA_TRY(cudaMemcpyAsync(sl.d_piece_out_start.p, ostart.data(), (size_t)mp * 8, cudaMemcpyHostToDevice, s_in));
         PIPE_CUDA_TRY(cudaMemcpyAsync(sl.d_piece_out_cap.p, ocap.data(), (size_t)mp * 4, cudaMemcpyHostToDevice, s_in));
@@ -537,7 +522,7 @@ static int ingest_core(xllm_ingest_t h, const xllm_ingest_io* io, const xllm_seg
     mark(4, s_out);
     sl.busy = true;
     h->last_chunks += 1;
-    h->last_launches += sp_encode_kernel_launches(h->sp_dev->dev(), h->memo_slots != 0, h->sp_warm) + (keys_stride > 0 || want_match ? 1 : 0) + (keys_stride > 0 ? 1 : 0) + (want_match ? 1 : 0);  // encode x2 or x3, prep, hash, match+route
+    h->last_launches += plan.kernels + (keys_stride > 0 || want_match ? 1 : 0) + (keys_stride > 0 ? 1 : 0) + (want_match ? 1 : 0);  // encode, prep, hash, match+route
     slot = (slot + 1) % n_slots;
     c0 = c1;
   }

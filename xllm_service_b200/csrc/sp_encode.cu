@@ -2447,8 +2447,6 @@ __global__ void __launch_bounds__(32, LONG ? 8 : ((MODE != 2 && !WARM) ? 16 : 27
 }  // namespace
 
 // ------------------------------------------------------------------------------ host side
-int g_warps_per_sm_override = 0;  // tuning knob (XLLM_SP_WARPS_PER_SM), 0 = fill shared memory
-
 #ifdef XLLM_EXP_STATS
 extern "C" void xllm_debug_exp_stats(unsigned long long* out) {
   cudaMemcpyFromSymbol(out, g_exp_stats, sizeof(unsigned long long) * kExpStats);
@@ -2577,7 +2575,6 @@ int SpDeviceModel::upload(const SpTables& t) {
   dev_.small_vocab = (t.n_pieces < 65535 && max_rank < 65535) ? 1 : 0;
   if (const char* w = getenv("XLLM_SP_FORCE_WIDE"))  // tests: run a small vocabulary through the 32-bit-state kernels
     if (atoi(w) != 0) dev_.small_vocab = 0;
-  if (const char* w = getenv("XLLM_SP_WARPS_PER_SM")) g_warps_per_sm_override = atoi(w);
   dev_.express = 1;
   if (const char* w = getenv("XLLM_SP_EXPRESS")) dev_.express = atoi(w) != 0 ? 1 : 0;   // 0: every window takes the buffer path
   // scratch pool for pre-tokens longer than the shared-memory paths hold
@@ -2619,206 +2616,179 @@ int SpDeviceModel::upload(const SpTables& t) {
   return XLLM_OK;
 }
 
+// Per device: the SM count, and the resident blocks per SM of the express kernel ([small_vocab]).
 static DeviceOnce g_sp_once;
+static int g_exp_per_sm[DeviceOnce::kMaxDevices][2];
 
 // Resident one-warp blocks per SM of a buffer-path kernel whose warp takes smem bytes of shared memory: as many as
-// 227 KB holds with 1 KB reserved per block, at most 27.  XLLM_SP_WARPS_PER_SM may lower it, except for Unigram.
-// The warm-up arena (sp_warm_arena_bytes) and the warm launch's grid are both sized from it.
-static int sp_warps_per_sm(const SpDev& dev, size_t smem) {
-  int w = (int)((227 * 1024) / (smem + 1024));
-  if (w > 27) w = 27;
-  if (!dev.unigram && g_warps_per_sm_override > 0 && g_warps_per_sm_override < w) w = g_warps_per_sm_override;
-  return w;
+// 227 KB holds with 1 KB reserved per block, at most 27.
+static int sp_warps_per_sm(size_t smem) {
+  const int w = (int)((227 * 1024) / (smem + 1024));
+  return w > 27 ? 27 : w;
 }
-
-static int sp_legacy_grid(const SpDev& dev, int n_req, bool warm = false) {
-  int n_sm = 0, d = 0;
-  if (cudaGetDevice(&d) != cudaSuccess || cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, d) != cudaSuccess)
-    return 0;
-  const bool small = dev.small_vocab != 0;
-  const bool hf = !warm;   // every buffer-path BPE kernel has 32-row columns; the warm-up kernels keep 16
-  const size_t smem = dev.unigram ? (small ? sizeof(WarpSmemUniT<true>) : sizeof(WarpSmemUniT<false>))
-                      : hf        ? (small ? sizeof(WarpSmemT<true, kHfRows>) : sizeof(WarpSmemT<false, kHfRows>))
-                                  : (small ? sizeof(WarpSmemT<true>) : sizeof(WarpSmemT<false>));
-  const int grid = n_sm * sp_warps_per_sm(dev, smem);
-  return grid > n_req ? n_req : grid;
-}
-size_t sp_warm_arena_bytes(const SpDev& dev, int n_req) { return (size_t)sp_legacy_grid(dev, n_req, true) * kWarmSliceBytes; }
 
 // the express kernel runs in front of the buffer-path kernel for these models (and only with the word memo on)
 static bool sp_express_model(const SpDev& dev) {
   return dev.express && !dev.unigram && !dev.byte_mode && dev.split_mode == 1 && dev.remove_extra_ws;
 }
-// blocks of kExpWarps warps the express kernel launches for n_req requests (resident blocks x SMs at most)
-static int sp_express_blocks(const SpDev& dev, int n_req) {
-  static int per_sm[2] = {0, 0};
+
+// One warp's shared memory in sp_encode_kernel<SMALL, ·, MODE, ·, WARM>: the kernel's own SM type.
+template <bool SMALL, int MODE, bool WARM>
+using EncodeSmem = typename std::conditional<MODE == 2, WarpSmemUniT<SMALL>, WarpSmemT<SMALL, WARM ? kMaxSym : kHfRows>>::type;
+
+template <bool SMALL>
+static size_t throughput_smem(bool unigram, bool warm) {
+  return unigram ? sizeof(EncodeSmem<SMALL, 2, false>)
+                 : (warm ? sizeof(EncodeSmem<SMALL, 0, true>) : sizeof(EncodeSmem<SMALL, 0, false>));
+}
+
+cudaError_t sp_encode_plan(const SpDev& dev, int n_req, bool memo, bool warm, SpEncodePlan* plan) {
+  SpEncodePlan& p = *plan;
+  p = SpEncodePlan();
+  cudaError_t e = cudaSuccess;
+  int d = 0;   // get() sets it before the setup runs
+  const int n_sm = g_sp_once.get(
+      [&] {
+        for (int s = 0; s < 2; ++s) {
+          int& b = g_exp_per_sm[d][s];
+          const cudaError_t r =
+              s ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, sp_express_kernel<true>, kExpWarps * 32,
+                                                                kExpWarps * sizeof(ExpSmemT<true>))
+                : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, sp_express_kernel<false>, kExpWarps * 32,
+                                                                kExpWarps * sizeof(ExpSmemT<false>));
+          if (r != cudaSuccess) return r;
+          if (b < 1) b = 1;
+        }
+        return cudaSuccess;
+      },
+      &e, &d);
+  if (e != cudaSuccess) return e;
   const bool small = dev.small_vocab != 0;
-  int n_sm = 0, d = 0;
-  if (cudaGetDevice(&d) != cudaSuccess || cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, d) != cudaSuccess)
-    return 0;
-  if (per_sm[small] == 0) {
-    int b = 0;
-    const cudaError_t e =
-        small ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, sp_express_kernel<true>, kExpWarps * 32,
-                                                              kExpWarps * sizeof(ExpSmemT<true>))
-              : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, sp_express_kernel<false>, kExpWarps * 32,
-                                                              kExpWarps * sizeof(ExpSmemT<false>));
-    per_sm[small] = (e == cudaSuccess && b > 0) ? b : 1;
+  const int n = n_req > 0 ? n_req : 0;
+  // the warm-up pre-passes live in the memo kernels of BPE models; the express kernel has none, so warm replaces it
+  p.memo = memo;
+  p.warm = warm && memo && !dev.unigram;
+  p.express = memo && !p.warm && sp_express_model(dev);
+  p.long_pass = !dev.unigram;   // Viterbi has no long-word pass
+  p.kernels = 1 + (p.express ? 1 : 0) + (p.long_pass ? 1 : 0);
+  const size_t smem = small ? throughput_smem<true>(dev.unigram, p.warm) : throughput_smem<false>(dev.unigram, p.warm);
+  const int full_grid = n_sm * sp_warps_per_sm(smem);
+  p.grid = full_grid < n ? full_grid : n;
+  p.grid_long = n_sm * 2 < n ? n_sm * 2 : n;
+  p.warp_ns = p.grid;
+  if (p.express) {
+    int per_sm = g_exp_per_sm[d][small];
+    if (const char* w = getenv("XLLM_SP_EXPRESS_BLOCKS_PER_SM")) {
+      const int v = atoi(w);
+      if (v > 0 && v < per_sm) per_sm = v;
+    }
+    const int need = (n + kExpWarps - 1) / kExpWarps;
+    p.express_blocks = n_sm * per_sm < need ? n_sm * per_sm : need;
+    if (p.express_blocks * kExpWarps > p.warp_ns) p.warp_ns = p.express_blocks * kExpWarps;
   }
-  int blocks = n_sm * per_sm[small];
-  if (const char* w = getenv("XLLM_SP_EXPRESS_BLOCKS_PER_SM")) {
-    const int v = atoi(w);
-    if (v > 0 && v < per_sm[small]) blocks = n_sm * v;
+  // scratch: [deferred requests n][handed-over requests n, to 16 bytes][resume records n]
+  p.scratch_bytes = (((size_t)n * 8 + 15) & ~(size_t)15) + (size_t)n * sizeof(ExpResume) + 16;
+  p.arena_bytes = p.warm ? (size_t)full_grid * kWarmSliceBytes : 0;
+  return cudaSuccess;
+}
+
+// What every kernel of one sp_encode_launch is passed.
+struct EncodeArgs {
+  const uint8_t* text;
+  const int64_t* offsets;
+  int n_req;
+  int32_t* ids;
+  int64_t ids_stride;
+  int32_t* n_ids;
+  int32_t* status;
+  SpDev dev;
+  unsigned int* counters;
+  void* scratch;
+  uint8_t* memo_table;
+  uint32_t memo_mask;
+  cudaStream_t stream;
+};
+
+// Launches sp_encode_kernel<SMALL, LONG, MODE, MEMO, WARM> with one warp per block and that warp's shared memory, the
+// size this instantiation is opted in to once per device.
+template <bool SMALL, bool LONG, int MODE, bool MEMO, bool WARM>
+static cudaError_t launch_encode(int grid, const EncodeArgs& a) {
+  constexpr size_t smem = sizeof(EncodeSmem<SMALL, MODE, WARM>);
+  static DeviceOnce once;
+  cudaError_t e = cudaSuccess;
+  once.get(
+      [] {
+        return cudaFuncSetAttribute(sp_encode_kernel<SMALL, LONG, MODE, MEMO, WARM>,
+                                    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      },
+      &e);
+  if (e != cudaSuccess) return e;
+  sp_encode_kernel<SMALL, LONG, MODE, MEMO, WARM><<<grid, 32, smem, a.stream>>>(
+      a.text, a.offsets, a.n_req, a.ids, a.ids_stride, a.n_ids, a.status, a.dev, a.counters + (LONG ? 2 : 0),
+      static_cast<int32_t*>(a.scratch), a.counters + 1, MEMO ? a.memo_table : nullptr, MEMO ? a.memo_mask : 0u);
+  return cudaGetLastError();
+}
+
+// BPE: the throughput kernel (memo off, on, or on with the warm-up pre-passes), then the long-word kernel over the
+// requests it deferred.
+template <bool SMALL, int MODE>
+static cudaError_t launch_bpe(const SpEncodePlan& p, const EncodeArgs& a) {
+  const cudaError_t e = p.warm   ? launch_encode<SMALL, false, MODE, true, true>(p.grid, a)
+                        : p.memo ? launch_encode<SMALL, false, MODE, true, false>(p.grid, a)
+                                 : launch_encode<SMALL, false, MODE, false, false>(p.grid, a);
+  if (e != cudaSuccess) return e;
+  return launch_encode<SMALL, true, MODE, false, false>(p.grid_long, a);
+}
+
+// Every kernel the plan lists, in order: the express kernel, whose hand-overs continue in the buffer-path kernels.
+template <bool SMALL>
+static cudaError_t launch_plan(const SpEncodePlan& p, EncodeArgs a) {
+  if (p.express) {
+    int32_t* const legacy_list = static_cast<int32_t*>(a.scratch) + a.n_req;
+    ExpResume* const resume =
+        reinterpret_cast<ExpResume*>(static_cast<uint8_t*>(a.scratch) + (((size_t)a.n_req * 8 + 15) & ~(size_t)15));
+    sp_express_kernel<SMALL><<<p.express_blocks, kExpWarps * 32, kExpWarps * sizeof(ExpSmemT<SMALL>), a.stream>>>(
+        a.text, a.offsets, a.n_req, a.ids, a.ids_stride, a.n_ids, a.status, a.dev, a.counters + 3, legacy_list,
+        a.counters + 4, resume, a.memo_table, a.memo_mask);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    a.dev.work_list = legacy_list;
+    a.dev.work_count = a.counters + 4;
+    a.dev.resume = resume;
   }
-  const int need = (n_req + kExpWarps - 1) / kExpWarps;
-  return blocks > need ? need : blocks;
+  // Unigram: Viterbi per word from a running score, so no word memo (the result depends on the prefix)
+  if (a.dev.unigram) return launch_encode<SMALL, false, 2, false, false>(p.grid, a);
+  return a.dev.split_mode == 3 ? launch_bpe<SMALL, 1>(p, a) : launch_bpe<SMALL, 0>(p, a);
 }
 
-int sp_encode_grid(const SpDev& dev, int n_req) {
-  const int legacy = sp_legacy_grid(dev, n_req);
-  const int express = sp_express_model(dev) ? sp_express_blocks(dev, n_req) * kExpWarps : 0;
-  return legacy > express ? legacy : express;
-}
-
-int sp_encode_kernel_launches(const SpDev& dev, bool memo_on, bool warm) {
-  return 2 + ((memo_on && !warm && sp_express_model(dev)) ? 1 : 0);
-}
-
-size_t sp_encode_scratch_bytes(int n_req) {
-  const size_t n = (size_t)(n_req > 0 ? n_req : 0);
-  return ((n * 8 + 15) & ~(size_t)15) + n * sizeof(ExpResume) + 16;
-}
-
-cudaError_t sp_encode_launch(const SpDev& dev_in, const uint8_t* text, const int64_t* offsets, int n_req, int32_t* ids,
+cudaError_t sp_encode_launch(const SpDev& dev, const uint8_t* text, const int64_t* offsets, int n_req, int32_t* ids,
                              int64_t ids_stride, int32_t* n_ids, int32_t* status, unsigned int* counters,
                              void* scratch, cudaStream_t stream, SpMemo memo, SpLaunchOpts opts) {
   if (n_req <= 0) return cudaSuccess;
-  DeviceOnce& once = g_sp_once;
-  SpDev dev = dev_in;   // the kernel takes the table descriptor by value: the per-launch options ride along
-  dev.out_start = opts.out_start;
-  dev.out_cap = opts.out_cap;
-  dev.warp_ns = opts.warp_ns;
-  dev.warm_arena = nullptr;
-  dev.work_list = nullptr;
-  dev.work_count = nullptr;
-  dev.resume = nullptr;
-  // scratch (sp_encode_scratch_bytes): [deferred requests n][handed-over requests n][resume records n]
-  int32_t* const defer_list = static_cast<int32_t*>(scratch);
-  int32_t* const legacy_list = defer_list + n_req;
-  ExpResume* const resume = reinterpret_cast<ExpResume*>(static_cast<uint8_t*>(scratch) + (((size_t)n_req * 8 + 15) & ~(size_t)15));
-  const bool small = dev.small_vocab != 0;
-  const bool hf = dev.split_mode == 3;
-  // the HF kernels (not their warm-up variants) use 32-row lane columns
-  const size_t smem16 = small ? sizeof(WarpSmemT<true>) : sizeof(WarpSmemT<false>);
-  const size_t smem_long = small ? sizeof(WarpSmemT<true, kHfRows>) : sizeof(WarpSmemT<false, kHfRows>);
-  cudaError_t e0 = cudaSuccess;
-  const int n_sm = once.get(
-      [&] {
-        cudaError_t r;
-#define XLLM_SET_SMEM(K, B)                                                                          \
-        r = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WarpSmemT<B>)); \
-        if (r != cudaSuccess) return r;
-#define XLLM_SET_SMEM_HF(K, B)                                                                                \
-        r = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WarpSmemT<B, kHfRows>)); \
-        if (r != cudaSuccess) return r;
-        XLLM_SET_SMEM_HF((sp_encode_kernel<true, false, 0, false>), true)
-        XLLM_SET_SMEM_HF((sp_encode_kernel<true, true, 0, false>), true)
-        XLLM_SET_SMEM_HF((sp_encode_kernel<false, false, 0, false>), false)
-        XLLM_SET_SMEM_HF((sp_encode_kernel<false, true, 0, false>), false)
-        XLLM_SET_SMEM_HF((sp_encode_kernel<true, false, 1, false>), true)
-        XLLM_SET_SMEM_HF((sp_encode_kernel<true, true, 1, false>), true)
-        XLLM_SET_SMEM_HF((sp_encode_kernel<false, false, 1, false>), false)
-        XLLM_SET_SMEM_HF((sp_encode_kernel<false, true, 1, false>), false)
-        XLLM_SET_SMEM_HF((sp_encode_kernel<true, false, 0, true>), true)
-        XLLM_SET_SMEM_HF((sp_encode_kernel<false, false, 0, true>), false)
-        XLLM_SET_SMEM_HF((sp_encode_kernel<true, false, 1, true>), true)
-        XLLM_SET_SMEM_HF((sp_encode_kernel<false, false, 1, true>), false)
-        XLLM_SET_SMEM((sp_encode_kernel<true, false, 0, true, true>), true)
-        XLLM_SET_SMEM((sp_encode_kernel<false, false, 0, true, true>), false)
-        XLLM_SET_SMEM((sp_encode_kernel<true, false, 1, true, true>), true)
-        XLLM_SET_SMEM((sp_encode_kernel<false, false, 1, true, true>), false)
-        r = cudaFuncSetAttribute(sp_encode_kernel<true, false, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)sizeof(WarpSmemUniT<true>));
-        if (r != cudaSuccess) return r;
-        r = cudaFuncSetAttribute(sp_encode_kernel<false, false, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)sizeof(WarpSmemUniT<false>));
-        if (r != cudaSuccess) return r;
-#undef XLLM_SET_SMEM
-#undef XLLM_SET_SMEM_HF
-        return cudaSuccess;
-      },
-      &e0);
-  if (e0 != cudaSuccess) return e0;
+  const bool use_memo = memo.table != nullptr && memo.slots >= 2 && (memo.slots & (memo.slots - 1)) == 0;
+  SpEncodePlan plan;
+  cudaError_t e = sp_encode_plan(dev, n_req, use_memo, memo.warm, &plan);
+  if (e != cudaSuccess) return e;
+  if (plan.warm && (memo.arena == nullptr || memo.arena_bytes < plan.arena_bytes)) return cudaErrorInvalidValue;
+  // the kernels take the table descriptor by value: the per-launch options ride along
+  EncodeArgs a{text, offsets, n_req, ids, ids_stride, n_ids, status, dev, counters, scratch,
+               plan.memo ? static_cast<uint8_t*>(memo.table) : nullptr, plan.memo ? memo.slots - 1 : 0u, stream};
+  a.dev.out_start = opts.out_start;
+  a.dev.out_cap = opts.out_cap;
+  a.dev.warp_ns = opts.warp_ns;
+  a.dev.warm_arena = plan.warm ? static_cast<uint8_t*>(memo.arena) : nullptr;
+  a.dev.work_list = nullptr;
+  a.dev.work_count = nullptr;
+  a.dev.resume = nullptr;
   // counters[0]: task counter, [1]: deferred count, [2]: task counter of the long-word pass,
   // [3]: task counter of the express kernel, [4]: requests it handed over
-  cudaError_t e = cudaMemsetAsync(counters, 0, 5 * sizeof(unsigned int), stream);
+  e = cudaMemsetAsync(counters, 0, 5 * sizeof(unsigned int), stream);
   if (e != cudaSuccess) return e;
-  auto grid_for = [&](size_t smem_bytes) {
-    const int g = n_sm * sp_warps_per_sm(dev, smem_bytes);
-    return g > n_req ? n_req : g;
-  };
-  int grid_long = n_sm * 2;
-  if (grid_long > n_req) grid_long = n_req;
-  const bool use_memo = memo.table != nullptr && memo.slots >= 2 && (memo.slots & (memo.slots - 1)) == 0;
   if (use_memo && memo.clear) {
     e = cudaMemsetAsync(memo.table, 0, (size_t)memo.slots * 32, stream);  // default policy: the memo lives for this launch only
     if (e != cudaSuccess) return e;
   }
-  // the warm-up kernels (drain_pass<..., WARM>) need their per-warp scratch; the caller passes it only when they are wanted
-  const bool warm = use_memo && !dev.unigram && memo.arena != nullptr &&
-                    memo.arena_bytes >= (size_t)grid_for(smem16) * kWarmSliceBytes;
-  const size_t smem = warm ? smem16 : smem_long;   // the throughput kernel's shared memory: 16-row columns when warm
-  const int grid = grid_for(smem);
-  if (warm) dev.warm_arena = static_cast<uint8_t*>(memo.arena);
-  uint8_t* const mt = use_memo ? static_cast<uint8_t*>(memo.table) : nullptr;
-  const uint32_t mm = use_memo ? memo.slots - 1 : 0;
-  // the express kernel first; what it cannot finish continues in the buffer-path kernel below (work list + resume records)
-  if (use_memo && !warm && sp_express_model(dev)) {
-    const int blocks = sp_express_blocks(dev, n_req);
-    if (small)
-      sp_express_kernel<true><<<blocks, kExpWarps * 32, kExpWarps * sizeof(ExpSmemT<true>), stream>>>(
-          text, offsets, n_req, ids, ids_stride, n_ids, status, dev, counters + 3, legacy_list, counters + 4, resume, mt, mm);
-    else
-      sp_express_kernel<false><<<blocks, kExpWarps * 32, kExpWarps * sizeof(ExpSmemT<false>), stream>>>(
-          text, offsets, n_req, ids, ids_stride, n_ids, status, dev, counters + 3, legacy_list, counters + 4, resume, mt, mm);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    dev.work_list = legacy_list;
-    dev.work_count = counters + 4;
-    dev.resume = resume;
-  }
-#define XLLM_LAUNCH_PAIR(SMALL_, HF_, MEMO_)                                                                     \
-  if (MEMO_ && warm)                                                                                             \
-    sp_encode_kernel<SMALL_, false, HF_, MEMO_, MEMO_><<<grid, 32, smem, stream>>>(                              \
-        text, offsets, n_req, ids, ids_stride, n_ids, status, dev, counters, defer_list, counters + 1, mt, mm);  \
-  else                                                                                                           \
-    sp_encode_kernel<SMALL_, false, HF_, MEMO_><<<grid, 32, smem, stream>>>(                                     \
-        text, offsets, n_req, ids, ids_stride, n_ids, status, dev, counters, defer_list, counters + 1, mt, mm);  \
-  sp_encode_kernel<SMALL_, true, HF_, false><<<grid_long, 32, smem_long, stream>>>(                              \
-      text, offsets, n_req, ids, ids_stride, n_ids, status, dev, counters + 2, defer_list, counters + 1, nullptr, 0u);
-  if (dev.unigram) {
-    // Viterbi per word from a running score: no word memo (the result depends on the prefix), no long-word pass
-    const size_t usmem = small ? sizeof(WarpSmemUniT<true>) : sizeof(WarpSmemUniT<false>);
-    const int ugrid = grid_for(usmem);
-    if (small)
-      sp_encode_kernel<true, false, 2, false><<<ugrid, 32, usmem, stream>>>(
-          text, offsets, n_req, ids, ids_stride, n_ids, status, dev, counters, defer_list, counters + 1, nullptr, 0u);
-    else
-      sp_encode_kernel<false, false, 2, false><<<ugrid, 32, usmem, stream>>>(
-          text, offsets, n_req, ids, ids_stride, n_ids, status, dev, counters, defer_list, counters + 1, nullptr, 0u);
-  } else if (use_memo) {
-    if (small && hf) { XLLM_LAUNCH_PAIR(true, 1, true) }
-    else if (small) { XLLM_LAUNCH_PAIR(true, 0, true) }
-    else if (hf) { XLLM_LAUNCH_PAIR(false, 1, true) }
-    else { XLLM_LAUNCH_PAIR(false, 0, true) }
-  } else {
-    if (small && hf) { XLLM_LAUNCH_PAIR(true, 1, false) }
-    else if (small) { XLLM_LAUNCH_PAIR(true, 0, false) }
-    else if (hf) { XLLM_LAUNCH_PAIR(false, 1, false) }
-    else { XLLM_LAUNCH_PAIR(false, 0, false) }
-  }
-#undef XLLM_LAUNCH_PAIR
-  return cudaGetLastError();
+  return dev.small_vocab ? launch_plan<true>(plan, a) : launch_plan<false>(plan, a);
 }
 
 }  // namespace xllm

@@ -104,31 +104,44 @@ struct SpMemo {
   // false: the launch reuses what earlier launches left in the table (same tokenizer model; entries are immutable, so a
   // stale table is only ever less complete) — the caller's policy decides when to clear (xllm_set_memo_policy)
   bool clear = true;
-  // scratch of the warm-up pre-passes (natural text: memo misses merged in full rounds, long words resolved ahead of
-  // the in-order rounds); at least sp_warm_arena_bytes(dev, n_req) bytes, or null to leave the pre-passes off
+  // true: run the warm-up pre-passes (natural text: memo misses merged in full rounds, long words resolved ahead of
+  // the in-order rounds); arena is their scratch, at least SpEncodePlan::arena_bytes
+  bool warm = false;
   void* arena = nullptr;
   size_t arena_bytes = 0;
 };
-size_t sp_warm_arena_bytes(const SpDev& dev, int n_req);
 uint32_t sp_memo_default_slots();  // XLLM_SP_MEMO_SLOTS (0 = off), default 2^18 = 8 MiB
+
+// What one sp_encode_launch over n_req requests runs, and the device memory it needs.
+struct SpEncodePlan {
+  bool memo = false;       // the throughput kernel uses the word memo
+  bool warm = false;       // ... with the warm-up pre-passes (BPE models, memo on)
+  bool express = false;    // the express kernel runs first (memo on, not warm, sp_express_model)
+  bool long_pass = false;  // the long-word kernel runs last, over the deferred requests (BPE models)
+  int kernels = 0;         // kernels enqueued
+  int express_blocks = 0;  // blocks of 4 warps
+  int grid = 0;            // warps (= blocks) of the buffer-path throughput kernel: as many as its shared memory lets
+                           // the SMs hold, at most n_req
+  int grid_long = 0;       // warps of the long-word kernel
+  int warp_ns = 0;         // SpLaunchOpts::warp_ns entries: the larger of the two throughput grids, in warps
+  size_t scratch_bytes = 0;  // sp_encode_launch's scratch
+  size_t arena_bytes = 0;    // warm: SpMemo::arena for the full grid (any n_req), else 0
+};
+cudaError_t sp_encode_plan(const SpDev& dev, int n_req, bool memo, bool warm, SpEncodePlan* plan);
 
 // text: all prompts back to back; offsets[n_req + 1] (bytes).  Request r's ids go to
 // ids + r * ids_stride (at most ids_stride of them), n_ids[r] = full count, status[r] = kEnc*.
-// counters: 8 uint32 in device memory; scratch: sp_encode_scratch_bytes(n_req) of device memory (work lists of the
-// follow-up kernels + resume records).  Launches: the express kernel (models it applies to, memo on), the
-// buffer-path throughput kernel over what is left, the long-word kernel over the deferred requests (no-op grids
-// when there is nothing to do).
+// counters: 8 uint32 in device memory; scratch: SpEncodePlan::scratch_bytes of device memory (work lists of the
+// follow-up kernels + resume records).  Launches the kernels sp_encode_plan lists (no-op grids when there is nothing
+// to do); a warm launch whose arena is smaller than the plan's fails with cudaErrorInvalidValue.
 struct SpLaunchOpts {
   // ragged output rows (text pieces of segmented requests, pipeline.cu): ids + out_start[r], capacity out_cap[r]
   const int64_t* out_start = nullptr;
   const int32_t* out_cap = nullptr;
-  // diagnostics: per-warp busy time of the throughput kernel's persistent grid ([grid] entries, see
-  // sp_encode_grid()); used by bench.py to report the length tail of variable-length batches
+  // diagnostics: per-warp busy time of the throughput kernels' persistent grids (SpEncodePlan::warp_ns entries);
+  // used by bench.py to report the length tail of variable-length batches
   unsigned long long* warp_ns = nullptr;
 };
-int sp_encode_grid(const SpDev& dev, int n_req);   // warps (= blocks) the throughput kernel launches for n_req requests
-int sp_encode_kernel_launches(const SpDev& dev, bool memo_on, bool warm);   // kernels one sp_encode_launch enqueues (2 or 3)
-size_t sp_encode_scratch_bytes(int n_req);          // device scratch one launch over n_req requests needs
 cudaError_t sp_encode_launch(const SpDev& dev, const uint8_t* text, const int64_t* offsets, int n_req, int32_t* ids,
                              int64_t ids_stride, int32_t* n_ids, int32_t* status, unsigned int* counters,
                              void* scratch, cudaStream_t stream, SpMemo memo = SpMemo(),
