@@ -1153,9 +1153,12 @@ __device__ unsigned long long g_exp_stats[kExpStats];
 
 // Runs express steps from source offset pos for as long as they apply; returns the offset reached and sets *failed
 // when it stopped in front of a window it cannot do (the caller sends that window through the buffer path).
-// Windows are 16-byte ALIGNED: the step loads the 32 aligned 16-byte units from the one that holds pos, turns the bytes
-// in front of pos (and past the end of the text) into spaces, and never consumes byte 511 of a window unless the text
-// ends inside it — so every consumed byte has its successor inside the window, where it was checked to be ASCII.
+// Windows are 16-byte ALIGNED: the step loads the 32 aligned 16-byte units from the one that holds the position, and
+// never consumes byte 511 of a window unless the text ends inside it — so every consumed byte has its successor inside
+// the window, where it was checked to be ASCII.  The bytes of the first unit in front of the position were consumed,
+// hence checked, by the step before (or by express_long_word): they stay as loaded and are masked out of the lane's
+// non-space bits.  Only foreign bytes are rewritten to spaces: those in front of the text in the request's first unit
+// (the previous request's, or nobody's) and those past the end of the text.  pos is 0 or where an earlier run stopped.
 struct ExpReq {
   const uint8_t* src;
   uint32_t len;
@@ -1276,11 +1279,19 @@ __device__ __forceinline__ uint32_t exp_blank(uint32_t x, int i, int lo, int hi)
   const uint32_t keep = below_b & ~below_a;
   return (x & keep) | (0x20202020u & ~keep);
 }
-// 0x80 in every space byte of x -> one bit per byte
-__device__ __forceinline__ uint32_t exp_space4(uint32_t x) {
-  x ^= 0x20202020u;
-  const uint32_t z = ~(((x & 0x7F7F7F7Fu) + 0x7F7F7F7Fu) | x | 0x7F7F7F7Fu);
-  return (((z >> 7) * 0x01020408u) >> 24) & 0xFu;
+// One bit per byte of x that is not a space.  Every byte of x is ASCII (< 0x80), so adding 0x7F to byte ^ 0x20 sets
+// the byte's high bit iff it is not zero, without a carry into the next byte.
+__device__ __forceinline__ uint32_t exp_nonspace4(uint32_t x) {
+  const uint32_t z = ((x ^ 0x20202020u) + 0x7F7F7F7Fu) & 0x80808080u;
+  return ((z >> 7) * 0x01020408u) >> 24;
+}
+// __ballot_sync(kFull, x & bit) with the bit test as one predicate-setting instruction (compiled from C++ the bit is
+// shifted down, masked and compared: three)
+__device__ __forceinline__ uint32_t exp_ballot_bit(uint32_t x, uint32_t bit) {
+  uint32_t r;
+  asm volatile("{ .reg .pred p; .reg .b32 t; and.b32 t, %1, %2; setp.ne.u32 p, t, 0; vote.sync.ballot.b32 %0, p, 0xffffffff; }"
+               : "=r"(r) : "r"(x), "r"(bit));
+  return r;
 }
 // The memo key (memo_key's layout) of the n <= 15 bytes of the window's text from offset s.
 __device__ __forceinline__ U128 exp_word_key(const uint4* txt, uint32_t s, int n, bool lead) {
@@ -1326,9 +1337,11 @@ __device__ __forceinline__ void exp_store(int32_t* out, U128 val, int cnt, int o
       }
     }
   } else {
+    // region: store-clipped (cold)
 #pragma unroll
     for (int q = 0; q < MemoIds<SMALL>::kMax; ++q)
       if (q < cnt && o + q < cap) out[o + q] = (int32_t)MemoIds<SMALL>::id(val, q);
+    // region: end
   }
 }
 
@@ -1367,12 +1380,15 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
     const uint32_t skip = v & 15u;
     const uint32_t wb = v - skip;                                  // the window's first (aligned) byte
     const bool at_end = wb + (uint32_t)kExpWin >= vlen;            // the text ends inside this window
-    if ((skip != 0u && lane == 0) || at_end) {                     // bytes in front of the position / past the end: spaces
-      const int lo = lane == 0 ? (int)skip : 0;
+    // region: blank
+    if (wb == 0u || at_end) {                                      // bytes in front of / past the end of the text: spaces
+      // region: blank-foreign (cold)
+      const int lo = wb == 0u && lane == 0 ? (int)skip : 0;
       const int hi = at_end ? (int)(vlen - wb) - 16 * lane : 16;
       w = make_uint4(exp_blank(w.x, 0, lo, hi), exp_blank(w.y, 1, lo, hi), exp_blank(w.z, 2, lo, hi),
                      exp_blank(w.w, 3, lo, hi));
     }
+    // region: classify
     {
       // every byte a simple ASCII byte (then it is its own unit, given an ASCII successor) or a space-like one
       bool ok = ((w.x | w.y | w.z | w.w) & 0x80808080u) == 0u;
@@ -1384,6 +1400,7 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
                   (((w.x + 0x01010101u) | (w.y + 0x01010101u) | (w.z + 0x01010101u) | (w.w + 0x01010101u)) &
                    0x80808080u) == 0u;                                                          // every byte <= 0x7E
       if (!__all_sync(kFull, ok && fast_ok)) {
+        // region: slow-classify (cold)
         uint32_t q[4] = {w.x, w.y, w.z, w.w};
 #pragma unroll
         for (int k = 0; k < 16; ++k) {
@@ -1397,10 +1414,12 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
         w = make_uint4(q[0], q[1], q[2], q[3]);
       }
     }
+    // region: starts
     EXP_CLOCK(t_vote);
-    // non-space bytes of the lane's 16 bytes; word starts / ends from the two neighbouring bytes
-    const uint32_t ns16 = ~(exp_space4(w.x) | (exp_space4(w.y) << 4) | (exp_space4(w.z) << 8) | (exp_space4(w.w) << 12)) &
-                          0xFFFFu;
+    // non-space bytes of the lane's 16 bytes, those in front of the position left out (consumed: simple bytes, or space-
+    // like ones the slow classification has turned into spaces again); word starts / ends from the two neighbouring bytes
+    const uint32_t ns16 = (exp_nonspace4(w.x) | (exp_nonspace4(w.y) << 4) | (exp_nonspace4(w.z) << 8) | (exp_nonspace4(w.w) << 12)) &
+                          (lane == 0 ? 0xFFFFu << skip : 0xFFFFu) & 0xFFFFu;
     sm.txt[lane] = w;                                              // the words' bytes are read from here
     uint32_t prev_ns = (__shfl_up_sync(kFull, ns16, 1) >> 15) & 1u;
     uint32_t next_ns = __shfl_down_sync(kFull, ns16, 1) & 1u;
@@ -1413,8 +1432,7 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
     const uint32_t en16 = ns16 & ~((ns16 >> 1) | (next_ns << 15)) & 0xFFFFu;
     // starts per lane: 0..8 (four bits) -> four ballots give every lane the index of its first start
     const uint32_t cs = __popc(st16);
-    const uint32_t b0 = __ballot_sync(kFull, cs & 1u), b1 = __ballot_sync(kFull, cs & 2u);
-    const uint32_t b2 = __ballot_sync(kFull, cs & 4u), b3 = __ballot_sync(kFull, cs & 8u);
+    const uint32_t b0 = exp_ballot_bit(cs, 1u), b1 = exp_ballot_bit(cs, 2u), b2 = exp_ballot_bit(cs, 4u), b3 = exp_ballot_bit(cs, 8u);
     const uint32_t last_ns = __ballot_sync(kFull, (ns16 & 0x8000u) != 0u) >> 31;
     const int nstart = __popc(b0) + 2 * __popc(b1) + 4 * __popc(b2) + 8 * __popc(b3);
     const int nend = nstart - (int)(at_end ? 0u : last_ns);       // an unfinished word at the end of the window
@@ -1422,6 +1440,7 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
     uint32_t cons = at_end ? vlen - wb : (uint32_t)kExpWin - 1u;   // window bytes consumed (counted from wb)
     bool S2 = true;
     uint4 w_next = make_uint4(0u, 0u, 0u, 0u);
+    // region: long-word (cold)
     // a word the lane path does not take, at window offset s0, through the cooperative path; false: the run stops
     // (the text is done, or the request is handed over at the word)
     auto long_word = [&](uint32_t s0) -> bool {
@@ -1451,15 +1470,18 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
       w = load_window(v);
       return true;
     };
+    // region: scatter
     if (nstart > 0) {
       {
         uint32_t k = __popc(b0 & lt) + 2 * __popc(b1 & lt) + 4 * __popc(b2 & lt) + 8 * __popc(b3 & lt);
         uint32_t e = k - (prev_ns & ns16 & 1u);    // words that ended before this lane = started - the one still open
+        // region: scatter-loop
         for (uint32_t m = st16; m && k <= (uint32_t)kExpWords; m &= m - 1u, ++k)
           ex[2u * k] = (uint16_t)(16 * lane + __ffs(m) - 1);
         for (uint32_t m = en16; m && e < (uint32_t)kExpWords; m &= m - 1u, ++e)
           ex[2u * e + 1u] = (uint16_t)(16 * lane + __ffs(m) - 1);
       }
+      // region: words
       __syncwarp();
       const bool inA = lane < take, inB = lane + 32 < take;
       const uint32_t seA = ex2[inA ? lane : 0], seB = ex2[inB ? lane + 32 : 0];
@@ -1471,6 +1493,7 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
       if (lmA) take = __ffs(lmA) - 1;
       else if (lmB) take = 32 + __ffs(lmB) - 1;
       if (take == 0) {
+        // region: first-word-long (cold)
         // the first word is long, or not finished inside this window
         const uint32_t s0 = ex[0];
         if (!lmA && s0 > skip) {
@@ -1482,11 +1505,13 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
           break;
         }
       } else {
+      // region: key
       const bool activeA = lane < take, activeB = lane + 32 < take;
       if (take < nstart) cons = ex[2 * take];      // stop in front of the first word not taken
       // --- the words' memo keys: {lead U+2581, length} byte + the word's bytes (all a miss needs later, too)
       const bool leadA = lane > 0 || P || (!S && sA > skip);       // word k + 32 always follows a kept space
       const U128 keyA = exp_word_key(sm.txt, sA, nA, leadA), keyB = exp_word_key(sm.txt, sB, nB, true);
+      // region: probe
       // --- memo: both words' first ways in flight before either is compared
       bool hitA = false, hitB = false;
       U128 valA{0ull, 0ull}, valB{0ull, 0ull};
@@ -1504,6 +1529,7 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
         if (activeA) hitA = exp_probe_finish<SMALL>(memo, keyA, slotA, kA, valA);
         if (activeB) hitB = exp_probe_finish<SMALL>(memo, keyB, slotB, kB, valB);
       }
+      // region: miss (cold)
       // --- misses: the merge of a drain round, from the bytes in registers, one word after the other
       bool hardA = false, hardB = false;
 #pragma unroll 1
@@ -1551,12 +1577,14 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
         if (h) hardB = hard;
         else hardA = hard;
       }
+      // region: hard-vote
       {
         // a word whose ids do not fit a memo payload: the words in front of it go out now, the word itself through
         // the cooperative path
         const uint32_t hmA = __ballot_sync(kFull, hardA), hmB = __ballot_sync(kFull, hardB);
         EXP_CLOCK(t_probe);
         if (hmA | hmB) {
+          // region: hard-word (cold)
           const int fh = hmA ? __ffs(hmA) - 1 : 32 + __ffs(hmB) - 1;
           EXP_STAT(8);
           if (fh == 0) {
@@ -1567,6 +1595,7 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
           cons = ex[2 * take];
         }
       }
+      // region: emit
       // the next window's bytes: in flight while this one's ids are stored (issued after the probes, so that its
       // registers are not live across them)
       w_next = load_window(wb + cons);
@@ -1579,8 +1608,8 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
       // lane its offsets
       const int cntA = lane < take ? MemoIds<SMALL>::count(valA) : 0;
       const int cntB = lane + 32 < take ? MemoIds<SMALL>::count(valB) : 0;
-      const uint32_t a0 = __ballot_sync(kFull, cntA & 1), a1 = __ballot_sync(kFull, cntA & 2), a2 = __ballot_sync(kFull, cntA & 4);
-      const uint32_t c0 = __ballot_sync(kFull, cntB & 1), c1 = __ballot_sync(kFull, cntB & 2), c2 = __ballot_sync(kFull, cntB & 4);
+      const uint32_t a0 = exp_ballot_bit(cntA, 1u), a1 = exp_ballot_bit(cntA, 2u), a2 = exp_ballot_bit(cntA, 4u);
+      const uint32_t c0 = exp_ballot_bit(cntB, 1u), c1 = exp_ballot_bit(cntB, 2u), c2 = exp_ballot_bit(cntB, 4u);
       const int totalA = __popc(a0) + 2 * __popc(a1) + 4 * __popc(a2);
       const int totalB = __popc(c0) + 2 * __popc(c1) + 4 * __popc(c2);
       const int oA = n_out + __popc(a0 & lt) + 2 * __popc(a1 & lt) + 4 * __popc(a2 & lt);
@@ -1598,6 +1627,7 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
     } else {
       w_next = load_window(wb + cons);
     }
+    // region: tail
     EXP_STAT(1);
     // --- the state a drain would have left: is_prev_space, and the U+2581 a kept space puts in front of the next word
     P = S2 && (take > 0 || P || !S);
@@ -1607,6 +1637,7 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
     w = w_next;
     __syncwarp();
   }
+  // region: end
 #ifdef XLLM_EXP_STATS
   if (lane == 0) {
     atomicAdd(&g_exp_stats[kExpStatTimed], n_timed);
