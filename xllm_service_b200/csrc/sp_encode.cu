@@ -1142,7 +1142,7 @@ __device__ int unigram_word_slow(const SpDev& T, SM& sm, const uint8_t* w, int l
 // ballot that first depends on the memo loads; emit: to after the id stores), summed per warp and added at the end.
 #ifdef XLLM_EXP_STATS
 constexpr int kExpStats = 32;
-enum : int { kExpStatTimed = 16, kExpStatCycWindow = 17, kExpStatCycProbe = 18, kExpStatCycEmit = 19 };
+enum : int { kExpStatScatterTrips = 3, kExpStatTimed = 16, kExpStatCycWindow = 17, kExpStatCycProbe = 18, kExpStatCycEmit = 19 };
 __device__ unsigned long long g_exp_stats[kExpStats];
 #define EXP_STAT(i) do { if (lane == 0) atomicAdd(&g_exp_stats[i], 1ull); } while (0)
 #define EXP_CLOCK(t) (t = clock64())
@@ -1169,14 +1169,14 @@ struct ExpReq {
   bool S;          // the normalizer's is_prev_space
   bool U;          // the last emitted symbol was unknown (matters with byte_fallback off only)
 };
-// per warp: symbol columns for the words the memo does not know yet, the window's text and its words' {start, end}
+// per warp: symbol columns for the words the memo does not know yet, the window's text and its words' owner lanes
 constexpr int kExpWords = 64;        // words an express step resolves: lane k takes words k and k + 32
 template <bool SMALL>
 struct ExpSmemT {
   uint32_t S[kMaxSym * 32];
   typename PMOps<SMALL>::T PM[kMaxSym * 32];
   uint4 txt[kExpWin / 16 + 1];       // the window (16 bytes per lane) + 16 bytes a word's key read may touch past it
-  uint16_t ex[2 * (kExpWords + 2)];  // {start, end} of words 0 .. kExpWords - 1, and the start of word kExpWords
+  uint8_t own[kExpWords];            // own[i]: the lane whose first start is word i (where some lane's is)
 };
 constexpr int kExpLongWords = 4;     // express_run: long words a request may put through the cooperative path ...
 constexpr int kExpLongEvery = 512;   // ... at a density above one per this many bytes before it is handed over
@@ -1285,6 +1285,38 @@ __device__ __forceinline__ uint32_t exp_nonspace4(uint32_t x) {
   const uint32_t z = ((x ^ 0x20202020u) + 0x7F7F7F7Fu) & 0x80808080u;
   return ((z >> 7) * 0x01020408u) >> 24;
 }
+// Entry b: the offsets of the set bits of b, four bits each from the lowest, in bits 0-15 as they are and in bits
+// 16-31 plus 8 (for the high byte of a lane's 16).  A byte holds at most four word starts (a start follows a space).
+struct ExpStartNibbles {
+  uint32_t v[256];
+};
+constexpr ExpStartNibbles exp_start_nibbles() {
+  ExpStartNibbles t{};
+  for (uint32_t b = 0; b < 256; ++b) {
+    uint32_t n = 0;
+    for (uint32_t i = 0; i < 8 && n < 4; ++i)
+      if ((b >> i) & 1u) {
+        t.v[b] |= (i << (4 * n)) | ((i + 8) << (4 * n + 16));
+        ++n;
+      }
+  }
+  return t;
+}
+// read through __ldg: the lanes read different entries, which the constant cache would serialise
+__device__ const ExpStartNibbles kExpStartNibbles = exp_start_nibbles();
+// The window offset of the start of word t (warp-uniform, below the window's count of starts), from the lanes'
+// non-space bits alone: for the steps that stop at a hard word, so that no word's start stays live across the probe
+__device__ __forceinline__ uint32_t exp_word_start(uint32_t ns16, uint32_t t, int lane) {
+  uint32_t prev = (__shfl_up_sync(kFull, ns16, 1) >> 15) & 1u;   // every lane takes part in the shuffle
+  if (lane == 0) prev = 0u;
+  uint32_t st = ns16 & ~((ns16 << 1) | prev) & 0xFFFFu;
+  const uint32_t c = __popc(st);
+  uint32_t r = t - (uint32_t)(warp_incl_scan((int)c, lane) - (int)c);   // the word's rank among this lane's starts
+  const int L = __ffs(__ballot_sync(kFull, r < c)) - 1;
+  if (r < c)
+    for (; r > 0u; --r) st &= st - 1u;
+  return __shfl_sync(kFull, 16u * lane + __ffs(st) - 1u, L);
+}
 // __ballot_sync(kFull, x & bit) with the bit test as one predicate-setting instruction (compiled from C++ the bit is
 // shifted down, masked and compared: three)
 __device__ __forceinline__ uint32_t exp_ballot_bit(uint32_t x, uint32_t bit) {
@@ -1359,8 +1391,6 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
   bool S = rs.S;
   bool U = rs.U;
   int n_long = 0;             // long words this request sent through the cooperative path
-  uint16_t* const ex = sm.ex;
-  const uint32_t* const ex2 = reinterpret_cast<const uint32_t*>(sm.ex);   // {start, end} of word k as one u32
   int32_t* const out = rs.out;
   const int32_t cap = rs.cap > 0x7fffffffll ? 0x7fffffff : (int32_t)rs.cap;
   int32_t n_out = (int32_t)rs.n_out;
@@ -1422,14 +1452,16 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
                           (lane == 0 ? 0xFFFFu << skip : 0xFFFFu) & 0xFFFFu;
     sm.txt[lane] = w;                                              // the words' bytes are read from here
     uint32_t prev_ns = (__shfl_up_sync(kFull, ns16, 1) >> 15) & 1u;
-    uint32_t next_ns = __shfl_down_sync(kFull, ns16, 1) & 1u;
+    uint32_t next16 = __shfl_down_sync(kFull, ns16, 1);
     if (lane == 0) prev_ns = 0u;
-    if (lane == 31) next_ns = at_end ? 0u : 1u;                    // unknown successor: the word is not complete
+    if (lane == 31) next16 = at_end ? 0u : 0xFFFFu;                // unknown successor: the word is not complete
+    // the lane's and its successor's non-space bits; bit 31 left clear, so that a word's end is found in them when it
+    // is at most 15 bytes long and a longer one shows as over 15
+    const uint32_t ns32 = ns16 | ((next16 & 0x7FFFu) << 16);
     if (!P && !S) {                                                // would continue a word that is not in the buffer
       if ((__shfl_sync(kFull, ns16, 0) >> skip) & 1u) { EXP_STAT(5); *failed = true; break; }
     }
     const uint32_t st16 = ns16 & ~((ns16 << 1) | prev_ns) & 0xFFFFu;
-    const uint32_t en16 = ns16 & ~((ns16 >> 1) | (next_ns << 15)) & 0xFFFFu;
     // starts per lane: 0..8 (four bits) -> four ballots give every lane the index of its first start
     const uint32_t cs = __popc(st16);
     const uint32_t b0 = exp_ballot_bit(cs, 1u), b1 = exp_ballot_bit(cs, 2u), b2 = exp_ballot_bit(cs, 4u), b3 = exp_ballot_bit(cs, 8u);
@@ -1470,24 +1502,43 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
       w = load_window(v);
       return true;
     };
-    // region: scatter
+    // region: select
     if (nstart > 0) {
+      // this lane's words are k .. k + cs - 1; offs: the in-lane offsets of their starts, four bits each
+      const uint32_t k = __popc(b0 & lt) + 2 * __popc(b1 & lt) + 4 * __popc(b2 & lt) + 8 * __popc(b3 & lt);
+      const uint32_t offs = (__ldg(&kExpStartNibbles.v[st16 & 0xFFu]) & 0xFFFFu) |
+                            ((__ldg(&kExpStartNibbles.v[st16 >> 8]) >> 16) << (4u * __popc(st16 & 0xFFu)));
+      // word j's owner is the lane whose k is the highest bit of M at or below j: M has bit k of every lane with a start
+      const bool owner = cs != 0u && k < (uint32_t)kExpWords;
+      if (owner) sm.own[k] = (uint8_t)lane;
+      const uint32_t kbit = owner ? 1u << (k & 31u) : 0u;
+      const uint32_t Mlo = __reduce_or_sync(kFull, k < 32u ? kbit : 0u), Mhi = __reduce_or_sync(kFull, k < 32u ? 0u : kbit);
+      const uint32_t le = (lt << 1) | 1u;
+      const uint32_t pA = 31 - __clz(Mlo & le), pB = (Mhi & le) ? 63 - __clz(Mhi & le) : 31 - __clz(Mlo);
+      // region: scatter-loop
+      // diagnostics build only: the trips of the two scatter loops this selection replaced (starts to k .. kExpWords,
+      // ends to e .. kExpWords - 1, each run as often as its busiest lane needs)
+#ifdef XLLM_EXP_STATS
       {
-        uint32_t k = __popc(b0 & lt) + 2 * __popc(b1 & lt) + 4 * __popc(b2 & lt) + 8 * __popc(b3 & lt);
-        uint32_t e = k - (prev_ns & ns16 & 1u);    // words that ended before this lane = started - the one still open
-        // region: scatter-loop
-        for (uint32_t m = st16; m && k <= (uint32_t)kExpWords; m &= m - 1u, ++k)
-          ex[2u * k] = (uint16_t)(16 * lane + __ffs(m) - 1);
-        for (uint32_t m = en16; m && e < (uint32_t)kExpWords; m &= m - 1u, ++e)
-          ex[2u * e + 1u] = (uint16_t)(16 * lane + __ffs(m) - 1);
+        const uint32_t e = k - (prev_ns & ns16 & 1u);
+        const uint32_t ce = __popc(ns16 & ~(ns32 >> 1) & 0xFFFFu);
+        const uint32_t t1 = k <= (uint32_t)kExpWords ? min(cs, (uint32_t)kExpWords + 1u - k) : 0u;
+        const uint32_t t2 = e < (uint32_t)kExpWords ? min(ce, (uint32_t)kExpWords - e) : 0u;
+        const uint32_t trips = __reduce_max_sync(kFull, t1) + __reduce_max_sync(kFull, t2);
+        if (lane == 0) atomicAdd(&g_exp_stats[kExpStatScatterTrips], (unsigned long long)trips);
       }
+#endif
       // region: words
       __syncwarp();
-      const bool inA = lane < take, inB = lane + 32 < take;
-      const uint32_t seA = ex2[inA ? lane : 0], seB = ex2[inB ? lane + 32 : 0];
-      const uint32_t sA = seA & 0xFFFFu, sB = seB & 0xFFFFu;
-      const int nA = (int)(seA >> 16) - (int)sA + 1, nB = (int)(seB >> 16) - (int)sB + 1;
+      const uint32_t oA = sm.own[pA], oB = sm.own[pB];
+      // a word's start from its rank among its owner's starts, its length from the owner's non-space bits (words
+      // past the last one get some offset of the window: their keys are never probed)
+      const uint32_t iA = __funnelshift_r(__shfl_sync(kFull, offs, oA), 0u, 4u * (lane - pA)) & 15u;
+      const uint32_t iB = __funnelshift_r(__shfl_sync(kFull, offs, oB), 0u, 4u * (lane + 32u - pB)) & 15u;
+      const uint32_t sA = 16u * oA + iA, sB = 16u * oB + iB;
+      const int nA = __ffs(~(__shfl_sync(kFull, ns32, oA) >> iA)) - 1, nB = __ffs(~(__shfl_sync(kFull, ns32, oB) >> iB)) - 1;
       // the lane path takes words of up to 15 bytes: stop in front of the first longer one (in text order)
+      const bool inA = lane < take, inB = lane + 32 < take;
       const uint32_t lmA = __ballot_sync(kFull, inA && nA > kMemoMaxKeyBytes);
       const uint32_t lmB = __ballot_sync(kFull, inB && nB > kMemoMaxKeyBytes);
       if (lmA) take = __ffs(lmA) - 1;
@@ -1495,7 +1546,7 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
       if (take == 0) {
         // region: first-word-long (cold)
         // the first word is long, or not finished inside this window
-        const uint32_t s0 = ex[0];
+        const uint32_t s0 = __shfl_sync(kFull, sA, 0);
         if (!lmA && s0 > skip) {
           cons = s0;                               // only spaces in front of it: take those, the word starts the next window
           w_next = load_window(wb + cons);
@@ -1507,7 +1558,10 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
       } else {
       // region: key
       const bool activeA = lane < take, activeB = lane + 32 < take;
-      if (take < nstart) cons = ex[2 * take];      // stop in front of the first word not taken
+      if (take < nstart) {                         // stop in front of the first word not taken (take <= kExpWords)
+        const uint32_t r = (uint32_t)take - k;
+        cons = __shfl_sync(kFull, 16u * lane + (__funnelshift_r(offs, 0u, 4u * r) & 15u), __ffs(__ballot_sync(kFull, r < cs)) - 1);
+      }
       // --- the words' memo keys: {lead U+2581, length} byte + the word's bytes (all a miss needs later, too)
       const bool leadA = lane > 0 || P || (!S && sA > skip);       // word k + 32 always follows a kept space
       const U128 keyA = exp_word_key(sm.txt, sA, nA, leadA), keyB = exp_word_key(sm.txt, sB, nB, true);
@@ -1587,12 +1641,13 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
           // region: hard-word (cold)
           const int fh = hmA ? __ffs(hmA) - 1 : 32 + __ffs(hmB) - 1;
           EXP_STAT(8);
+          const uint32_t sh = exp_word_start(ns16, (uint32_t)fh, lane);
           if (fh == 0) {
-            if (long_word(ex[0])) continue;
+            if (long_word(sh)) continue;
             break;
           }
           take = fh;
-          cons = ex[2 * take];
+          cons = sh;
         }
       }
       // region: emit
