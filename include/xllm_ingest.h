@@ -212,7 +212,10 @@ int xllm_score_route_device(xllm_ingest_t h, int32_t n_req, const uint64_t* d_ma
  * XLLM_ENC_TRUNCATED (count > ids_stride: call again with a larger stride),
  * XLLM_ERR_CAPACITY (a single pre-token longer than the device scratch holds) or, on the HF backend,
  * XLLM_ERR_INVALID_ARG (malformed UTF-8: the reference's Rust shim panics there, lib.rs:91) or
- * XLLM_ERR_UNSUPPORTED (tokenizer.json with normalizer NFC and a text that is not provably in NFC already).
+ * XLLM_ERR_UNSUPPORTED (tokenizer.json with normalizer NFC and a text that is not provably in NFC already: under
+ * the default XLLM_NFC_PROVE_INERT any char that is not NFC-inert; under XLLM_NFC_VERIFY a text that is not in NFC,
+ * or one whose run of chars after a boundary char that holds an NFC_Quick_Check = Maybe char is longer than 32 code
+ * points — see xllm_set_nfc_policy).  A refused request has n_ids = 0 and is never tokenised un-normalised.
  * An empty prompt yields 0 ids (sentencepiece_tokenizer.cpp:117-120) plus, on the HF backend, the
  * template's special tokens.
  * Backend, in the order of TokenizerFactory::create_tokenizer (tokenizer_factory.cpp:9-32):
@@ -299,6 +302,22 @@ int xllm_set_pipeline(xllm_ingest_t h, int32_t chunk_requests, int64_t chunk_byt
  * the service setting (host/ingest_batcher.h): small batches no longer pay for the cold table, results are identical
  * either way (a stale table is only ever less complete).  Env XLLM_SP_MEMO_PERSIST=N sets it at create. */
 int xllm_set_memo_policy(xllm_ingest_t h, int64_t persist_requests);
+/* Tokenizers with `normalizer: NFC` (Qwen2 / Qwen2.5 / Qwen3 tokenizer.json): the device never normalises, it
+ * tokenises a request as is only when NFC provably leaves it unchanged, and refuses the others per request with
+ * XLLM_ERR_UNSUPPORTED (a caller hands those to a CPU tokenizer).  How it proves it:
+ *   XLLM_NFC_PROVE_INERT (default): every char is NFC-inert (ccc 0, unchanged by NFC, never the second half of a
+ *     composition).  Refuses most text in scripts with combining marks (Thai, Devanagari, Bengali, Arabic with
+ *     harakat, ...) even when it is in NFC.
+ *   XLLM_NFC_VERIFY: an exact check ahead of the tokenizer kernels (UAX #15 quick check, completed by normalising the
+ *     chunks it answers "maybe" for).  Every text in NFC is accepted, except that a chunk holding an NFC_Quick_Check =
+ *     Maybe char — a boundary char (ccc 0, NFC_QC Yes) or the text start, then the run of non-boundary chars — is
+ *     refused when longer than 32 code points.  Malformed UTF-8 still gives XLLM_ERR_INVALID_ARG, first.  One more
+ *     kernel per launch.
+ * Other values: XLLM_ERR_INVALID_ARG.  No effect on models without `normalizer: NFC`.  Env XLLM_HF_NFC_VERIFY=1 sets
+ * XLLM_NFC_VERIFY at create; xllm_ingest_clone copies the policy. */
+#define XLLM_NFC_PROVE_INERT 0
+#define XLLM_NFC_VERIFY 1
+int xllm_set_nfc_policy(xllm_ingest_t h, int32_t policy);
 /* Chunks and kernel launches of the most recent xllm_ingest_batch on this handle (for launch accounting). */
 int xllm_last_batch_stats(xllm_ingest_t h, int32_t* n_chunks, int32_t* n_kernel_launches);
 /* Page-locked host memory for the batch buffers. */

@@ -84,6 +84,7 @@ class Segments(ctypes.Structure):
 
 
 _VP = ctypes.c_void_p
+NFC_PROVE_INERT, NFC_VERIFY = 0, 1   # xllm_set_nfc_policy (include/xllm_ingest.h)
 
 
 def _declare(L):
@@ -124,6 +125,7 @@ def _declare(L):
     L.xllm_index_export.argtypes = [_VP, ctypes.c_int64, _VP, _VP, _VP, _VP, ctypes.POINTER(ctypes.c_int64)]
     L.xllm_set_pipeline.argtypes = [_VP, ctypes.c_int32, ctypes.c_int64]
     L.xllm_set_memo_policy.argtypes = [_VP, ctypes.c_int64]
+    L.xllm_set_nfc_policy.argtypes = [_VP, ctypes.c_int32]
     L.xllm_last_batch_stats.argtypes = [_VP, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32)]
     L.xllm_host_alloc.argtypes = [ctypes.POINTER(_VP), ctypes.c_size_t]
     L.xllm_host_free.argtypes = [_VP]

@@ -61,7 +61,8 @@ void PinBuf::release() {
 
 int encode_reserve(xllm_ingest* h, int n_req, DevBuf* scratch, DevBuf* memo_buf, int64_t* memo_age, SpMemo* memo,
                    SpEncodePlan* plan) {
-  XLLM_CUDA_TRY(sp_encode_plan(h->sp_dev->dev(), n_req, h->memo_slots != 0, h->sp_warm, plan));
+  XLLM_CUDA_TRY(sp_encode_plan(h->sp_dev->dev(), n_req, h->memo_slots != 0, h->sp_warm, plan,
+                               h->nfc_policy == XLLM_NFC_VERIFY));
   XLLM_TRY_RC(scratch->reserve(plan->scratch_bytes));
   *memo = SpMemo();
   if (plan->memo) {
@@ -137,6 +138,7 @@ int xllm_ingest_create(const xllm_ingest_config* cfg, xllm_ingest_t* out) {
     h->memo_slots = sp_memo_default_slots();
     if (const char* w = getenv("XLLM_SP_MEMO_PERSIST")) h->memo_persist_requests = atoll(w) > 0 ? atoll(w) : 0;
     if (const char* w = getenv("XLLM_SP_WARM")) h->sp_warm = atoi(w) != 0;
+    if (const char* w = getenv("XLLM_HF_NFC_VERIFY")) h->nfc_policy = atoi(w) != 0 ? XLLM_NFC_VERIFY : XLLM_NFC_PROVE_INERT;
     if (const char* w = getenv("XLLM_PIPE_SLOTS")) {
       const int v = atoi(w);
       if (v >= 1 && v <= kPipeSlots) h->pipe_slots = v;
@@ -206,6 +208,7 @@ int xllm_ingest_clone(xllm_ingest_t src, xllm_ingest_t* out) {
   (*out)->sp_dev = src->sp_dev;
   (*out)->memo_slots = src->memo_slots;
   (*out)->memo_persist_requests = src->memo_persist_requests;
+  (*out)->nfc_policy = src->nfc_policy;
   (*out)->sp_warm = src->sp_warm;
   (*out)->pipe_slots = src->pipe_slots;
   (*out)->tokenizer_path = src->tokenizer_path;
@@ -696,8 +699,10 @@ int xllm_encode_batch_device(xllm_ingest_t h, int32_t n_req, const uint8_t* d_te
   SpMemo memo;
   SpEncodePlan plan;
   XLLM_TRY_RC(encode_reserve(h, n_req, &h->d_defer, &h->d_memo, &h->memo_age, &memo, &plan));
+  SpLaunchOpts opts;
+  opts.nfc_verify = plan.nfc_verify;
   XLLM_CUDA_TRY(sp_encode_launch(h->sp_dev->dev(), d_text, d_offsets, n_req, d_ids, ids_stride, d_n_ids, d_status,
-                                 h->d_task_counter + 4, h->d_defer.p, s, memo));
+                                 h->d_task_counter + 4, h->d_defer.p, s, memo, opts));
   return XLLM_OK;
 }
 
@@ -738,6 +743,7 @@ static int encode_batch_impl(xllm_ingest_t h, int32_t n_req, const uint8_t* text
     XLLM_CUDA_TRY(cudaMemcpyAsync(h->d_text.p, text + offsets[0], text_bytes, cudaMemcpyHostToDevice, s));
   XLLM_CUDA_TRY(cudaMemcpyAsync(h->d_offsets.p, offsets, (size_t)(n_req + 1) * 8, cudaMemcpyHostToDevice, s));
   SpLaunchOpts opts;
+  opts.nfc_verify = plan.nfc_verify;
   const int grid = plan.warp_ns;
   if (warp_ns) {   // diagnostics: per-warp busy time of the persistent grid
     XLLM_TRY_RC(h->d_masks.reserve((size_t)grid * 8 + 8));

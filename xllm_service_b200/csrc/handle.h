@@ -97,6 +97,7 @@ struct xllm_ingest {
   xllm::DevBuf d_memo;      // word memo of the single-launch encode entry points
   int64_t memo_age = -1;    // requests encoded since d_memo was last cleared; -1 = never
   int64_t memo_persist_requests = 0;  // 0: every launch clears its memo; N > 0: a memo is kept until it has seen N requests
+  int32_t nfc_policy = 0;   // XLLM_NFC_PROVE_INERT / XLLM_NFC_VERIFY (xllm_set_nfc_policy; normalizer-NFC models only)
   xllm::DevBuf d_arena;     // warm-up scratch of the encode kernel (per handle: launches on one handle are serialised)
   uint32_t memo_slots = 0;  // 0 = memo off
   bool sp_warm = false;     // XLLM_SP_WARM=1: launch the warm-up tokenizer kernels (natural text; sp_encode.cu drain_pass, WARM)
@@ -108,7 +109,8 @@ struct xllm_ingest {
 namespace xllm {
 // Plans one sp_encode_launch over n_req rows on handle h and reserves what it needs: the launch scratch, the word memo
 // table and the warm-up arena.  memo_buf / memo_age: the handle's or the pipeline slot's table and its age
-// (xllm_set_memo_policy), which this launch advances.  Fills *memo for the launch.
+// (xllm_set_memo_policy), which this launch advances.  Fills *memo for the launch; the plan follows the handle's NFC
+// policy, so the launch passes SpLaunchOpts::nfc_verify = plan->nfc_verify.
 int encode_reserve(xllm_ingest* h, int n_req, DevBuf* scratch, DevBuf* memo_buf, int64_t* memo_age, SpMemo* memo,
                    SpEncodePlan* plan);
 }  // namespace xllm

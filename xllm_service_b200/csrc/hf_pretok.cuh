@@ -168,7 +168,7 @@ __device__ HfScan hf_scan(const SpDev& T, SM& sm, int nlen, bool final, int lane
                               : l == 3 ? (((b0 & 0x0Fu) << 12) | ((nb[p + 1] & 0x3Fu) << 6) | (nb[p + 2] & 0x3Fu))
                                        : (((b0 & 0x07u) << 18) | ((nb[p + 1] & 0x3Fu) << 12) | ((nb[p + 2] & 0x3Fu) << 6) | (nb[p + 3] & 0x3Fu));
             const uint8_t tb = hf_class(T, cp);   // bits 0-1 class, 2 NFC-suspect, 3-4: 1 P, 2 S, 3 M (class 0 only)
-            nfc_bad |= T.nfc_check && (tb & kUniNfcSuspect);
+            nfc_bad |= T.nfc_check && !T.nfc_verdict && (tb & kUniNfcSuspect);   // verified: hf_nfc.cu
             v = tb & 3;
             if (p3) {
               const uint8_t sub = (tb >> 3) & 3;

@@ -437,11 +437,14 @@ static int ingest_core(xllm_ingest_t h, const xllm_ingest_io* io, const xllm_seg
     // ---- kernels: tokenize -> row prep -> chained block hash -> index probe -> match scan + routing
     PIPE_CUDA_TRY(cudaStreamWaitEvent(s_k, sl.ev[0], 0));
     if (!seg) {
+      xllm::SpLaunchOpts opts;
+      opts.nfc_verify = plan.nfc_verify;
       PIPE_CUDA_TRY(sp_encode_launch(h->sp_dev->dev(), sl.d_text.as<uint8_t>() - t0, sl.d_offsets.as<int64_t>(), m,
                                      sl.d_ids.as<int32_t>(), io->ids_stride, sl.d_n_ids.as<int32_t>(),
-                                     sl.d_status.as<int32_t>(), sl.counters, sl.d_defer.p, s_k, memo));
+                                     sl.d_status.as<int32_t>(), sl.counters, sl.d_defer.p, s_k, memo, opts));
     } else {
       xllm::SpLaunchOpts opts;
+      opts.nfc_verify = plan.nfc_verify;
       opts.out_start = sl.d_piece_out_start.as<int64_t>();
       opts.out_cap = sl.d_piece_out_cap.as<int32_t>();
       PIPE_CUDA_TRY(sp_encode_launch(h->sp_dev->dev(), sl.d_text.as<uint8_t>() - t0, sl.d_offsets.as<int64_t>(), mp,
@@ -578,6 +581,16 @@ int xllm_set_memo_policy(xllm_ingest_t h, int64_t persist_requests) {
   if (!h || persist_requests < 0) return XLLM_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(h->mu);
   h->memo_persist_requests = persist_requests;
+  return XLLM_OK;
+}
+
+int xllm_set_nfc_policy(xllm_ingest_t h, int32_t policy) {
+  if (!h || (policy != XLLM_NFC_PROVE_INERT && policy != XLLM_NFC_VERIFY)) {
+    xllm::set_last_error("xllm_set_nfc_policy: invalid argument");
+    return XLLM_ERR_INVALID_ARG;
+  }
+  std::lock_guard<std::mutex> lock(h->mu);
+  h->nfc_policy = policy;
   return XLLM_OK;
 }
 

@@ -42,6 +42,7 @@
 
 #include "common.cuh"
 #include "sp_long_word.cuh"
+#include "unicode_nfc.inc"   // host side: uploaded for normalizer-NFC models (SpDeviceModel::upload)
 
 namespace xllm {
 
@@ -2408,11 +2409,16 @@ __global__ void __launch_bounds__(32, LONG ? 8 : ((MODE != 2 && !WARM) ? 16 : 27
     rs.long_n = 0;
 
     if constexpr (HF) {
+      // a request the NFC verify kernel refused is not tokenised: malformed UTF-8, else not in NFC
+      if (T.nfc_verdict) {
+        const uint8_t v = T.nfc_verdict[r];
+        if (v) rs.bad_input = v == 2 ? 1 : 2;
+      }
       // TemplateProcessing ids in front (add_special_tokens = 1, fast_tokenizer.cpp:24), also for an empty text
       if (lane < T.n_prefix) put_id(rs, lane, T.prefix_ids[lane]);
       rs.n_out = T.n_prefix;
       if (lane == 0) sm.wstart[0] = 0;
-      for (uint32_t pos = 0; pos < rs.len; pos += kFastWin) {
+      for (uint32_t pos = 0; pos < rs.len && !rs.bad_input; pos += kFastWin) {
         normalize_fast(T, sm, rs, pos, lane);  // byte mode: a verbatim copy
         if (rs.nlen > drain_at) {
           drain<SMALL, LONG, 1, MEMO, WARM>(T, sm, rs, false, lane, memo);
@@ -2636,6 +2642,17 @@ int SpDeviceModel::upload(const SpTables& t) {
     dev_.vtab_mask = (uint32_t)(t.vocab_table.size() / 4) - 1;
   }
   dev_.nfc_check = t.nfc_check ? 1 : 0;
+  if (t.nfc_check) {   // the tables of the exact NFC check (hf_nfc.cu), generated by scripts/gen_unicode_nfc.py
+    if ((rc = up(kNfcStage1, sizeof(kNfcStage1), reinterpret_cast<const void**>(&dev_.nfc1))) != XLLM_OK ||
+        (rc = up(kNfcStage2, sizeof(kNfcStage2), reinterpret_cast<const void**>(&dev_.nfc2))) != XLLM_OK ||
+        (rc = up(kNfcDecompCp, sizeof(kNfcDecompCp), reinterpret_cast<const void**>(&dev_.nfc_decomp_cp))) != XLLM_OK ||
+        (rc = up(kNfcDecomp, sizeof(kNfcDecomp), reinterpret_cast<const void**>(&dev_.nfc_decomp))) != XLLM_OK ||
+        (rc = up(kNfcCompKey, sizeof(kNfcCompKey), reinterpret_cast<const void**>(&dev_.nfc_comp_key))) != XLLM_OK ||
+        (rc = up(kNfcComp, sizeof(kNfcComp), reinterpret_cast<const void**>(&dev_.nfc_comp))) != XLLM_OK)
+      return rc;
+    dev_.n_nfc_decomp = (uint32_t)(sizeof(kNfcDecompCp) / sizeof(kNfcDecompCp[0]));
+    dev_.n_nfc_comp = (uint32_t)(sizeof(kNfcComp) / sizeof(kNfcComp[0]));
+  }
   dev_.hf_pattern = (uint8_t)t.hf_pattern;
   dev_.hf_digits = (uint8_t)(t.hf_digits > 0 ? t.hf_digits : 1);
   dev_.n_prefix = (uint8_t)t.prefix_ids.size();
@@ -2728,7 +2745,14 @@ static size_t throughput_smem(bool unigram, bool warm) {
                  : (warm ? sizeof(EncodeSmem<SMALL, 0, true>) : sizeof(EncodeSmem<SMALL, 0, false>));
 }
 
-cudaError_t sp_encode_plan(const SpDev& dev, int n_req, bool memo, bool warm, SpEncodePlan* plan) {
+// where the NFC verdicts start in the launch scratch: after the work lists and resume records
+static size_t nfc_verdict_offset(int n) {
+  return ((((size_t)n * 8 + 15) & ~(size_t)15) + (size_t)n * sizeof(ExpResume) + 16 + 15) & ~(size_t)15;
+}
+// resident blocks of hf_nfc_verify_kernel per SM (its __launch_bounds__ minimum)
+constexpr int kNfcBlocksPerSm = 8;
+
+cudaError_t sp_encode_plan(const SpDev& dev, int n_req, bool memo, bool warm, SpEncodePlan* plan, bool nfc_verify) {
   SpEncodePlan& p = *plan;
   p = SpEncodePlan();
   cudaError_t e = cudaSuccess;
@@ -2775,6 +2799,14 @@ cudaError_t sp_encode_plan(const SpDev& dev, int n_req, bool memo, bool warm, Sp
   // scratch: [deferred requests n][handed-over requests n, to 16 bytes][resume records n]
   p.scratch_bytes = (((size_t)n * 8 + 15) & ~(size_t)15) + (size_t)n * sizeof(ExpResume) + 16;
   p.arena_bytes = p.warm ? (size_t)full_grid * kWarmSliceBytes : 0;
+  // NFC verification: one more kernel ahead of the rest, its verdicts after the scratch above
+  p.nfc_verify = nfc_verify && dev.nfc_check && dev.split_mode == 3;
+  if (p.nfc_verify) {
+    p.kernels += 1;
+    const int need = (n + kNfcWarps - 1) / kNfcWarps;
+    p.nfc_blocks = n_sm * kNfcBlocksPerSm < need ? n_sm * kNfcBlocksPerSm : need;
+    p.scratch_bytes = nfc_verdict_offset(n) + (size_t)n + 16;
+  }
   return cudaSuccess;
 }
 
@@ -2853,7 +2885,7 @@ cudaError_t sp_encode_launch(const SpDev& dev, const uint8_t* text, const int64_
   if (n_req <= 0) return cudaSuccess;
   const bool use_memo = memo.table != nullptr && memo.slots >= 2 && (memo.slots & (memo.slots - 1)) == 0;
   SpEncodePlan plan;
-  cudaError_t e = sp_encode_plan(dev, n_req, use_memo, memo.warm, &plan);
+  cudaError_t e = sp_encode_plan(dev, n_req, use_memo, memo.warm, &plan, opts.nfc_verify);
   if (e != cudaSuccess) return e;
   if (plan.warm && (memo.arena == nullptr || memo.arena_bytes < plan.arena_bytes)) return cudaErrorInvalidValue;
   // the kernels take the table descriptor by value: the per-launch options ride along
@@ -2866,13 +2898,20 @@ cudaError_t sp_encode_launch(const SpDev& dev, const uint8_t* text, const int64_
   a.dev.work_list = nullptr;
   a.dev.work_count = nullptr;
   a.dev.resume = nullptr;
+  a.dev.nfc_verdict = nullptr;
   // counters[0]: task counter, [1]: deferred count, [2]: task counter of the long-word pass,
-  // [3]: task counter of the express kernel, [4]: requests it handed over
-  e = cudaMemsetAsync(counters, 0, 5 * sizeof(unsigned int), stream);
+  // [3]: task counter of the express kernel, [4]: requests it handed over, [5]: task counter of the NFC verify kernel
+  e = cudaMemsetAsync(counters, 0, (plan.nfc_verify ? 6 : 5) * sizeof(unsigned int), stream);
   if (e != cudaSuccess) return e;
   if (use_memo && memo.clear) {
     e = cudaMemsetAsync(memo.table, 0, (size_t)memo.slots * 32, stream);  // default policy: the memo lives for this launch only
     if (e != cudaSuccess) return e;
+  }
+  if (plan.nfc_verify) {
+    uint8_t* verdict = static_cast<uint8_t*>(scratch) + nfc_verdict_offset(n_req);
+    e = hf_nfc_verify_launch(dev, text, offsets, n_req, verdict, counters + 5, plan.nfc_blocks, stream);
+    if (e != cudaSuccess) return e;
+    a.dev.nfc_verdict = verdict;
   }
   return dev.small_vocab ? launch_plan<true>(plan, a) : launch_plan<false>(plan, a);
 }

@@ -59,10 +59,22 @@ struct SpDev {
   uint32_t max_piece_len;
   const uint4* utrie;   // byte trie of the pieces: {parent, byte, child, piece id or -1}, parent 0xFFFFFFFF = empty
   uint32_t utrie_mask;
-  uint8_t nfc_check;   // normalizer NFC: a request passes only if every char is NFC-inert (then NFC is the identity)
+  uint8_t nfc_check;   // normalizer NFC: a request passes only if NFC provably leaves it unchanged: every char is
+                       // NFC-inert, or (nfc_verdict set) the verify kernel found it in NFC
+  // normalizer NFC, exact verification (hf_nfc.cu; uploaded for nfc_check models, scripts/gen_unicode_nfc.py):
+  // {ccc, NFC_Quick_Check} per code point (two-stage), full canonical decompositions, primary composites
+  const uint16_t* nfc1;
+  const uint16_t* nfc2;
+  const uint32_t* nfc_decomp_cp;         // ascending
+  const uint32_t* nfc_decomp;            // 4 per entry, 0-padded
+  const unsigned long long* nfc_comp_key;  // first << 21 | second, ascending
+  const uint32_t* nfc_comp;
+  uint32_t n_nfc_decomp, n_nfc_comp;
   uint8_t hf_pattern;  // 1: ByteLevel's own GPT-2 regex, 2: Split(cl100k-family regex) + ByteLevel(use_regex = false)
   uint8_t hf_digits;   // pattern 2: \p{N}{1,hf_digits}
   // per-launch options (set by sp_encode_launch from SpLaunchOpts; null = off)
+  const uint8_t* nfc_verdict;    // [n_req] verdicts of hf_nfc_verify_kernel (0 NFC, 1 not NFC, 2 malformed UTF-8):
+                                 // the inert-char proof is skipped and a refused request is not tokenised
   const int64_t* out_start;      // request r's ids go to ids + out_start[r] (at most out_cap[r]) instead of r * ids_stride
   const int32_t* out_cap;
   unsigned long long* warp_ns;   // [grid]: nanoseconds each warp of the throughput kernel spent from start to exit
@@ -81,6 +93,7 @@ constexpr int32_t kEncOk = 0;
 constexpr int32_t kEncTruncated = 1;     // more ids than ids_stride: n_ids holds the full count, the row its prefix
 constexpr int32_t kEncBadUtf8 = -1;      // HF backend: the text is not valid UTF-8 (the reference's Rust shim panics)
 constexpr int32_t kEncNeedsNfc = -5;     // HF backend with normalizer NFC: the text is not provably in NFC (XLLM_ERR_UNSUPPORTED)
+                                         // or, verifying, not in NFC / holds a Maybe chunk over kNfcChunkCap code points
 constexpr int32_t kEncWordTooLong = -6;  // a single pre-token exceeds the on-chip word capacity (XLLM_ERR_CAPACITY)
 
 class SpDeviceModel {
@@ -91,7 +104,7 @@ class SpDeviceModel {
 
  private:
   SpDev dev_{};
-  void* allocs_[24] = {nullptr};
+  void* allocs_[32] = {nullptr};
   int n_allocs_ = 0;
 };
 
@@ -124,10 +137,13 @@ struct SpEncodePlan {
                            // the SMs hold, at most n_req
   int grid_long = 0;       // warps of the long-word kernel
   int warp_ns = 0;         // SpLaunchOpts::warp_ns entries: the larger of the two throughput grids, in warps
-  size_t scratch_bytes = 0;  // sp_encode_launch's scratch
+  bool nfc_verify = false; // hf_nfc_verify_kernel runs first (asked for, and the model has normalizer NFC)
+  int nfc_blocks = 0;      // its blocks of kNfcWarps warps
+  size_t scratch_bytes = 0;  // sp_encode_launch's scratch (+ one verdict byte per request when nfc_verify)
   size_t arena_bytes = 0;    // warm: SpMemo::arena for the full grid (any n_req), else 0
 };
-cudaError_t sp_encode_plan(const SpDev& dev, int n_req, bool memo, bool warm, SpEncodePlan* plan);
+cudaError_t sp_encode_plan(const SpDev& dev, int n_req, bool memo, bool warm, SpEncodePlan* plan,
+                           bool nfc_verify = false);
 
 // text: all prompts back to back; offsets[n_req + 1] (bytes).  Request r's ids go to
 // ids + r * ids_stride (at most ids_stride of them), n_ids[r] = full count, status[r] = kEnc*.
@@ -141,10 +157,21 @@ struct SpLaunchOpts {
   // diagnostics: per-warp busy time of the throughput kernels' persistent grids (SpEncodePlan::warp_ns entries);
   // used by bench.py to report the length tail of variable-length batches
   unsigned long long* warp_ns = nullptr;
+  // normalizer NFC: verify each request exactly (hf_nfc.cu) instead of proving every char NFC-inert
+  // (xllm_set_nfc_policy); no effect on other models.  Plan with the same flag.
+  bool nfc_verify = false;
 };
 cudaError_t sp_encode_launch(const SpDev& dev, const uint8_t* text, const int64_t* offsets, int n_req, int32_t* ids,
                              int64_t ids_stride, int32_t* n_ids, int32_t* status, unsigned int* counters,
                              void* scratch, cudaStream_t stream, SpMemo memo = SpMemo(),
                              SpLaunchOpts opts = SpLaunchOpts());
+
+// Exact NFC verification (hf_nfc.cu): one warp per request, blocks of kNfcWarps warps; verdict[r] = 0 in NFC, 1 not in
+// NFC or a chunk holding an NFC_QC = Maybe char is longer than kNfcChunkCap code points, 2 malformed UTF-8.
+// task_counter: one zeroed uint32 in device memory.
+constexpr int kNfcChunkCap = 32;
+constexpr int kNfcWarps = 4;
+cudaError_t hf_nfc_verify_launch(const SpDev& dev, const uint8_t* text, const int64_t* offsets, int n_req,
+                                 uint8_t* verdict, unsigned int* task_counter, int blocks, cudaStream_t stream);
 
 }  // namespace xllm

@@ -35,6 +35,10 @@
 
 #include "xllm_ingest.h"
 
+// Weak: a program that links the batcher against an older build of the library (or a stand-in for the C-ABI without
+// this entry point) still links; the handle then keeps its default NFC policy.
+extern "C" int xllm_set_nfc_policy(xllm_ingest_t h, int32_t policy) __attribute__((weak));
+
 namespace xllm_host {
 
 struct IngestResult {
@@ -56,6 +60,9 @@ class IngestBatcher {
     // a service's batches are small and come one after the other: keep the tokenizer's word memo across launches
     // (cleared every memo_persist_requests requests) instead of starting every batch from an empty table
     xllm_set_memo_policy(h, memo_persist_requests);
+    // tokenizers with `normalizer: NFC` (Qwen2 family): accept every request that is in NFC, not only those made of
+    // NFC-inert chars, so text with combining marks (Thai, Devanagari, ...) stays on the device
+    if (xllm_set_nfc_policy) xllm_set_nfc_policy(h, XLLM_NFC_VERIFY);
     // vocabularies below 65 536 pieces: take the ids as uint16 (half the bytes over PCIe) and widen them in hand_out,
     // during the copy into the caller's std::vector<int32_t> that happens anyway
     int32_t vocab = 0;

@@ -49,6 +49,8 @@ class GpuTokenizer final : public Tokenizer {
     cfg.xxh3_seed = seed;
     cfg.device = device;
     CHECK_EQ(xllm_ingest_create(&cfg, &h_), XLLM_OK) << xllm_last_error();
+    // normalizer NFC: serve every request that is in NFC on the device; only text NFC would change goes to fallback_
+    xllm_set_nfc_policy(h_, XLLM_NFC_VERIFY);
     legacy_ = tokenizers_new_from_path(dir_.c_str());  // decode / vocabulary queries
   }
   GpuTokenizer(xllm_ingest_t cloned, const std::string& dir, std::unique_ptr<Tokenizer> fallback)

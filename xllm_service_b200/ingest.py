@@ -276,6 +276,11 @@ class Ingest:
         """0: every encode launch clears its word memo (default); N > 0: a memo is kept until it has seen N requests."""
         check(self._L.xllm_set_memo_policy(self._h, persist_requests))
 
+    def set_nfc_policy(self, policy):
+        """Tokenizers with `normalizer: NFC`: 0 (XLLM_NFC_PROVE_INERT, default) accepts a request only when every char
+        is NFC-inert; 1 (XLLM_NFC_VERIFY) checks exactly whether it is in NFC.  Refused requests get status -5."""
+        check(self._L.xllm_set_nfc_policy(self._h, policy))
+
     def last_batch_stats(self):
         """(chunks, kernel launches) of the most recent ingest_batch on this handle."""
         c, k = ctypes.c_int32(), ctypes.c_int32()
