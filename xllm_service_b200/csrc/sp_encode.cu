@@ -1176,6 +1176,7 @@ template <bool SMALL>
 struct ExpSmemT {
   uint32_t S[kMaxSym * 32];
   typename PMOps<SMALL>::T PM[kMaxSym * 32];
+  uint4 txt_front;                   // read (and masked off) by the key of a word at the window's first byte
   uint4 txt[kExpWin / 16 + 1];       // the window (16 bytes per lane) + 16 bytes a word's key read may touch past it
   uint8_t own[kExpWords];            // own[i]: the lane whose first start is word i (where some lane's is)
 };
@@ -1326,54 +1327,73 @@ __device__ __forceinline__ uint32_t exp_ballot_bit(uint32_t x, uint32_t bit) {
                : "=r"(r) : "r"(x), "r"(bit));
   return r;
 }
-// The memo key (memo_key's layout) of the n <= 15 bytes of the window's text from offset s.
-__device__ __forceinline__ U128 exp_word_key(const uint4* txt, uint32_t s, int n, bool lead) {
-  const uint2* t8 = reinterpret_cast<const uint2*>(txt) + (s >> 3);
-  const uint2 u0 = t8[0], u1 = t8[1], u2 = t8[2];
-  const bool odd = (s & 4u) != 0u;
-  const uint32_t bsh = (s & 3u) * 8u;
-  const uint32_t t0 = odd ? u0.y : u0.x, t1 = odd ? u1.x : u0.y, t2 = odd ? u1.y : u1.x, t3 = odd ? u2.x : u1.y,
-                 t4 = odd ? u2.y : u2.x;
-  unsigned long long lo = (unsigned long long)__funnelshift_r(t0, t1, bsh) | ((unsigned long long)__funnelshift_r(t1, t2, bsh) << 32);
-  unsigned long long hi = (unsigned long long)__funnelshift_r(t2, t3, bsh) | ((unsigned long long)__funnelshift_r(t3, t4, bsh) << 32);
-  if (n < 8) { lo &= (1ull << (8 * n)) - 1ull; hi = 0ull; }
-  else hi &= (1ull << (8 * (n - 8))) - 1ull;
-  return U128{(lo << 8) | (unsigned long long)((lead ? 0x80u : 0u) | (uint32_t)n), (hi << 8) | (lo >> 56)};
+// Entry n: the byte masks of a memo key with n word bytes (bytes 1 .. n kept, the header byte 0 cleared); entries
+// past 15 serve the keys computed for words that are not taken (up to 31 bytes: their lengths come from 32 bits).
+struct ExpKeyMasks {
+  uint4 v[32];
+};
+constexpr ExpKeyMasks exp_key_masks() {
+  ExpKeyMasks t{};
+  for (int n = 0; n < 32; ++n) {
+    uint32_t m[4] = {0, 0, 0, 0};
+    for (int j = 1; j <= n && j < 16; ++j) m[j >> 2] |= 0xFFu << (8 * (j & 3));
+    t.v[n] = uint4{m[0], m[1], m[2], m[3]};
+  }
+  return t;
 }
-// The memo probe's second half: compare the first way loaded by the caller, load the second way when the first holds
-// another word.  Returns hit (a key match with ids); val holds the payload of the way that matched.  Both ways are
-// loaded with ld_b128_cached: the hot words' slots stay in the SM's L1, which takes the L2 round trip off most
-// probes, the longest link of a step.  A slot read before another SM's insert reaches it reads as a miss: the lane
-// merges the word, and its insert's CAS, which goes to L2, finds the key there.
+__device__ const ExpKeyMasks kExpKeyMasks = exp_key_masks();
+// The memo key (memo_key's layout) of the n <= 15 bytes of the window's text from offset s: the 16 bytes from s - 1
+// (byte 0 becomes the header) funnel-shifted out of five 32-bit words, the bytes past the word masked off.
+__device__ __forceinline__ U128 exp_word_key(const uint4* txt, uint32_t s, int n, bool lead) {
+  const uint32_t* t = reinterpret_cast<const uint32_t*>(txt) - 1 + ((s + 3u) >> 2);   // the word holding byte s - 1
+  const uint32_t bsh = ((s + 3u) & 3u) * 8u;
+  const uint4 m = __ldg(&kExpKeyMasks.v[n]);
+  const uint32_t t0 = t[0], t1 = t[1], t2 = t[2], t3 = t[3], t4 = t[4];
+  const uint32_t k0 = (__funnelshift_r(t0, t1, bsh) & m.x) | (lead ? 0x80u : 0u) | (uint32_t)n;
+  const uint32_t k1 = __funnelshift_r(t1, t2, bsh) & m.y, k2 = __funnelshift_r(t2, t3, bsh) & m.z,
+                 k3 = __funnelshift_r(t3, t4, bsh) & m.w;
+  return U128{(unsigned long long)k0 | ((unsigned long long)k1 << 32), (unsigned long long)k2 | ((unsigned long long)k3 << 32)};
+}
+// The memo probe's second half: compare the first way loaded by the caller, load the second way when the first does
+// not hold the word with its ids.  Returns hit (a key match with ids); val holds the payload of the second way when
+// the first missed.  Both ways are loaded with ld_b128_cached: the hot words' slots stay in the SM's L1, which takes
+// the L2 round trip off most probes, the longest link of a step.  A slot read before another SM's insert reaches it
+// reads as a miss: the lane merges the word, and its insert's CAS, which goes to L2, finds the key there.  An empty
+// first way (the word is not in the table) is not told apart: that miss costs a second load, the hits none.  Nor is
+// a first way with the word's key and zero ids: the second way cannot hold the word (an insert stops at the first way
+// that is empty or holds it), so it reads as a miss as well.
+template <bool SMALL>
+__device__ __forceinline__ bool exp_way_hit(U128 key, U128 k, U128 val) {
+  // the key's xor and the valid bit's absence in one word: one test
+  const uint32_t bad = ((uint32_t)k.lo ^ (uint32_t)key.lo) | ((uint32_t)(k.lo >> 32) ^ (uint32_t)(key.lo >> 32)) |
+                       ((uint32_t)k.hi ^ (uint32_t)key.hi) | ((uint32_t)(k.hi >> 32) ^ (uint32_t)(key.hi >> 32)) |
+                       (~(uint32_t)val.lo & (SMALL ? 0x8000u : 0x80000000u));
+  return bad == 0u;
+}
 template <bool SMALL>
 __device__ __forceinline__ bool exp_probe_finish(MemoRef memo, U128 key, uint32_t slot, U128 k, U128& val) {
-  if (k.lo == key.lo && k.hi == key.hi) return MemoIds<SMALL>::valid(val);
-  if ((k.lo | k.hi) == 0) return false;
+  if (exp_way_hit<SMALL>(key, k, val)) return true;
   const uint8_t* e = memo.table + (size_t)(slot ^ 1u) * 32;
   const U128 k2 = ld_b128_cached(e);
   val = ld_b128_cached(e + 16);
-  return k2.lo == key.lo && k2.hi == key.hi && MemoIds<SMALL>::valid(val);
+  return exp_way_hit<SMALL>(key, k2, val);
 }
-// A word's ids from its memo payload at out[o ..]; c1 / c2: some lane of the warp has a word of >= 2 / >= 4 ids.
+// A word's ids from its memo payload at p[0 ..]: the lane's own run of cnt ids, each store predicated on the lane's
+// count alone (no warp-wide "some lane has >= 2 / >= 4 ids" gates: with 64 words a step they are open in most steps,
+// and the gated form measured slower).  room: the ids the row still holds from p on.
 template <bool SMALL>
-__device__ __forceinline__ void exp_store(int32_t* out, U128 val, int cnt, int o, bool c1, bool c2, bool fits,
-                                          int32_t cap) {
+__device__ __forceinline__ void exp_store(int32_t* p, U128 val, int cnt, bool fits, int room) {
   if (fits) {      // the whole step fits the row (always, but for a truncating ids_stride)
-    if (cnt >= 1) out[o] = (int32_t)MemoIds<SMALL>::id(val, 0);
-    if (c1 || c2) {
-      if (cnt >= 2) out[o + 1] = (int32_t)MemoIds<SMALL>::id(val, 1);
-      if (cnt >= 3) out[o + 2] = (int32_t)MemoIds<SMALL>::id(val, 2);
-      if (c2) {
+    const uint32_t run = (1u << cnt) - 1u;   // bit q: the word has an id q (the bits set the store predicates at once)
+    if (cnt > 0) p[0] = (int32_t)MemoIds<SMALL>::id(val, 0);
 #pragma unroll
-        for (int q = 3; q < MemoIds<SMALL>::kMax; ++q)
-          if (q < cnt) out[o + q] = (int32_t)MemoIds<SMALL>::id(val, q);
-      }
-    }
+    for (int q = 1; q < MemoIds<SMALL>::kMax; ++q)
+      if ((run >> q) & 1u) p[q] = (int32_t)MemoIds<SMALL>::id(val, q);
   } else {
     // region: store-clipped (cold)
 #pragma unroll
     for (int q = 0; q < MemoIds<SMALL>::kMax; ++q)
-      if (q < cnt && o + q < cap) out[o + q] = (int32_t)MemoIds<SMALL>::id(val, q);
+      if (q < cnt && q < room) p[q] = (int32_t)MemoIds<SMALL>::id(val, q);
     // region: end
   }
 }
@@ -1392,7 +1412,10 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
   bool S = rs.S;
   bool U = rs.U;
   int n_long = 0;             // long words this request sent through the cooperative path
-  int32_t* const out = rs.out;
+  // the row's address held as one 64-bit value: an id's address is then one wide multiply-add from it (rebuilt from
+  // the kernel's ids parameter and a 64-bit row index, it takes four instructions per word)
+  int32_t* out = rs.out;
+  asm("" : "+l"(out));
   const int32_t cap = rs.cap > 0x7fffffffll ? 0x7fffffff : (int32_t)rs.cap;
   int32_t n_out = (int32_t)rs.n_out;
   const uint32_t lt = (1u << lane) - 1u;
@@ -1668,11 +1691,12 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
       const uint32_t c0 = exp_ballot_bit(cntB, 1u), c1 = exp_ballot_bit(cntB, 2u), c2 = exp_ballot_bit(cntB, 4u);
       const int totalA = __popc(a0) + 2 * __popc(a1) + 4 * __popc(a2);
       const int totalB = __popc(c0) + 2 * __popc(c1) + 4 * __popc(c2);
-      const int oA = n_out + __popc(a0 & lt) + 2 * __popc(a1 & lt) + 4 * __popc(a2 & lt);
-      const int oB = n_out + totalA + __popc(c0 & lt) + 2 * __popc(c1 & lt) + 4 * __popc(c2 & lt);
+      const int oA = __popc(a0 & lt) + 2 * __popc(a1 & lt) + 4 * __popc(a2 & lt);     // from n_out
+      const int oB = totalA + __popc(c0 & lt) + 2 * __popc(c1 & lt) + 4 * __popc(c2 & lt);
       const bool fits = n_out + totalA + totalB <= cap;
-      exp_store<SMALL>(out, valA, cntA, oA, a1 != 0u, a2 != 0u, fits, cap);
-      if (c0 | c1 | c2) exp_store<SMALL>(out, valB, cntB, oB, c1 != 0u, c2 != 0u, fits, cap);
+      int32_t* const row = out + n_out;
+      exp_store<SMALL>(row + oA, valA, cntA, fits, cap - n_out - oA);
+      if (c0 | c1 | c2) exp_store<SMALL>(row + oB, valB, cntB, fits, cap - n_out - oB);
       n_out += totalA + totalB;
       U = false;
 #ifdef XLLM_EXP_STATS
