@@ -275,7 +275,7 @@ def seq3(c):
 
 
 def rules3(c):
-    """position-local rules + scanned facts (what csrc/hf_pretok.cuh evaluates for hf_pattern 3)"""
+    """position-local rules + scanned facts (what csrc/hf_pretok.cuh hf_rules3 evaluates)"""
     n, k = len(c), [kind3(x) for x in c]
     nl = [x in "\r\n" for x in c]
     # an ASCII punctuation char that opens "punct + ASCII letters": it must be a token start itself (the previous char

@@ -158,6 +158,17 @@ def test_hf_tokenizer_json_tables(tmp_path):
             d[path[-1]] = value
         return f
 
+    def pre_of(style):
+        with open(os.path.join(HERE, "golden", style, "tokenizer.json")) as f:
+            return json.load(f)["pre_tokenizer"]
+
+    def sequence(pre, edit):   # another fixture's pre_tokenizer Sequence, its entries edited
+        def f(d):
+            d["pre_tokenizer"] = json.loads(json.dumps(pre))
+            edit(d["pre_tokenizer"]["pretokenizers"])
+        return f
+
+    cl100k, deepseek = pre_of("hf_llama3_style"), pre_of("hf_deepseek_style")
     for name, edit in (
         ("nfkc", set_(["normalizer"], {"type": "NFKC"})),
         ("other_regex", set_(["pre_tokenizer"], {"type": "Sequence", "pretokenizers": [
@@ -167,6 +178,12 @@ def test_hf_tokenizer_json_tables(tmp_path):
         ("prefix_space", set_(["pre_tokenizer", "add_prefix_space"], True)),
         ("no_regex", set_(["pre_tokenizer", "use_regex"], False)),
         ("whitespace", set_(["pre_tokenizer"], {"type": "Whitespace"})),
+        ("cl100k_merged", sequence(cl100k, lambda s: s[0].__setitem__("behavior", "MergedWithPrevious"))),
+        ("cl100k_invert", sequence(cl100k, lambda s: s[0].__setitem__("invert", True))),
+        ("cl100k_byte_level_regex", sequence(cl100k, lambda s: s[1].__setitem__("use_regex", True))),
+        ("deepseek_order", sequence(deepseek, lambda s: s.insert(0, s.pop(1)))),
+        ("deepseek_no_byte_level", sequence(deepseek, lambda s: s.pop())),
+        ("byte_level_alone", sequence(cl100k, lambda s: s.pop(0))),
         ("wordpiece", set_(["model", "type"], "WordPiece")),
         ("truncation", set_(["truncation"], {"max_length": 8, "strategy": "LongestFirst", "stride": 0, "direction": "Right"})),
         ("lstrip", lambda d: d["added_tokens"][0].__setitem__("lstrip", True)),
@@ -186,6 +203,9 @@ def test_hf_tokenizer_json_tables(tmp_path):
     assert _lib.tokenizer_probe(variant("im", set_(["model", "ignore_merges"], True)))["split_mode"] == 3
     for style in ("hf_llama3_style", "hf_qwen2_style"):
         assert _lib.tokenizer_probe(os.path.join(HERE, "golden", style))["split_mode"] == 3
+    # ... and the refused sequences above are refused for their edit alone
+    for name, pre in (("cl100k", cl100k), ("deepseek", deepseek)):
+        assert _lib.tokenizer_probe(variant(name, sequence(pre, lambda s: None)))["split_mode"] == 3
     # a template post-processor is accepted (ids are wrapped on device)
     tp = {"type": "TemplateProcessing",
           "single": [{"SpecialToken": {"id": "<|endoftext|>", "type_id": 0}}, {"Sequence": {"id": "A", "type_id": 0}}],

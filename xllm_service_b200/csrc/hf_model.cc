@@ -7,7 +7,8 @@
 //
 // Supported configuration (everything else fails the load with XLLM_ERR_UNSUPPORTED — never a silent
 // approximation): model BPE without dropout / unk / prefix / suffix / byte_fallback / ignore_merges;
-// normalizer null; pre_tokenizer ByteLevel{add_prefix_space:false, use_regex:true} (the GPT-2 pattern);
+// normalizer null; pre_tokenizer one of the layouts in hf_load_model's kLayouts (GPT-2 ByteLevel, cl100k-family
+// Split, DeepSeek-V3's three Splits);
 // post_processor null, ByteLevel, or a TemplateProcessing whose `single` template only wraps the sequence in
 // special tokens; added tokens that are matched verbatim (normalized:false, no lstrip/rstrip/single_word).
 // Tables: byte_mode (every byte is a symbol: the byte-level alphabet is a bijection byte <-> char), the pair
@@ -16,6 +17,7 @@
 #include <string.h>
 #include <sys/stat.h>
 
+#include <algorithm>
 #include <string>
 #include <unordered_map>
 #include <utility>
@@ -189,6 +191,27 @@ bool flag_false_or_absent(const JVal* o, const char* key) {
   return !v || v->is_null() || (v->type == JVal::kBool && !v->b);
 }
 
+// pre_tokenizer ByteLevel{add_prefix_space: false} with use_regex (default true) as wanted
+bool byte_level_ok(const JVal& bl, bool want_regex) {
+  const JVal* bt = bl.get("type");
+  const JVal* rx = bl.get("use_regex");
+  const bool use_regex = !(rx && rx->type == JVal::kBool && !rx->b);
+  return bt && bt->type == JVal::kStr && bt->str == "ByteLevel" && flag_false_or_absent(&bl, "add_prefix_space") &&
+         use_regex == want_regex;
+}
+
+// pre_tokenizer Split{pattern: {Regex}, behavior: Isolated, invert: false} -> its regex; null for any other entry
+const std::string* split_regex(const JVal& sp) {
+  const JVal* st = sp.get("type");
+  const JVal* pat = sp.get("pattern");
+  const JVal* rx = pat ? pat->get("Regex") : nullptr;
+  const JVal* beh = sp.get("behavior");
+  if (!st || st->type != JVal::kStr || st->str != "Split" || !rx || rx->type != JVal::kStr || !beh ||
+      beh->type != JVal::kStr || beh->str != "Isolated" || !flag_false_or_absent(&sp, "invert"))
+    return nullptr;
+  return &rx->str;
+}
+
 }  // namespace
 
 // The top-level string member `key` of a JSON file, as the reference's JsonReader::value<std::string>(key) reads it
@@ -278,55 +301,40 @@ int hf_load_model(const std::string& path_in, SpTables* t) {
         "(?i:'s|'t|'re|'ve|'m|'ll|'d)|[^\\r\\n\\p{L}\\p{N}]?\\p{L}+|\\p{N}{1,3}| ?[^\\s\\p{L}\\p{N}]+[\\r\\n]*|\\s*[\\r\\n]+|\\s+(?!\\S)|\\s+";
     static const char* kP1 =
         "(?i:'s|'t|'re|'ve|'m|'ll|'d)|[^\\r\\n\\p{L}\\p{N}]?\\p{L}+|\\p{N}| ?[^\\s\\p{L}\\p{N}]+[\\r\\n]*|\\s*[\\r\\n]+|\\s+(?!\\S)|\\s+";
-    const JVal* ty = pre ? pre->get("type") : nullptr;
-    if (!ty || ty->type != JVal::kStr) return fail(t, XLLM_ERR_UNSUPPORTED, kUnsupported);
-    auto byte_level_ok = [&](const JVal* bl, bool want_regex) {
-      const JVal* bt = bl->get("type");
-      const JVal* rx = bl->get("use_regex");
-      const bool use_regex = !(rx && rx->type == JVal::kBool && !rx->b);
-      return bt && bt->type == JVal::kStr && bt->str == "ByteLevel" && flag_false_or_absent(bl, "add_prefix_space") &&
-             use_regex == want_regex;
+    // the accepted layouts: the Split regexes in order, then ByteLevel, with its own regex only when there is no Split
+    struct Layout {
+      size_t n_splits;
+      const char* splits[3];
+      int pattern, digits;
     };
-    if (ty->str == "ByteLevel") {
-      if (!byte_level_ok(pre, true)) return fail(t, XLLM_ERR_UNSUPPORTED, kUnsupported);
-      t->hf_pattern = 1;
-    } else if (ty->str == "Sequence") {
-      const JVal* seq = pre->get("pretokenizers");
-      if (seq && seq->type == JVal::kArr && seq->arr.size() == 4) {
-        const char* want[3] = {kDs1, kDs2, kDs3};
-        for (int k = 0; k < 3; ++k) {
-          const JVal& sp = seq->arr[(size_t)k];
-          const JVal* st = sp.get("type");
-          const JVal* pat = sp.get("pattern");
-          const JVal* rx = pat ? pat->get("Regex") : nullptr;
-          const JVal* beh = sp.get("behavior");
-          if (!st || st->type != JVal::kStr || st->str != "Split" || !rx || rx->type != JVal::kStr || !beh ||
-              beh->type != JVal::kStr || beh->str != "Isolated" || !flag_false_or_absent(&sp, "invert") ||
-              rx->str != want[k])
-            return fail(t, XLLM_ERR_UNSUPPORTED, std::string(kUnsupported) + (rx && rx->type == JVal::kStr ? "; got regex " + rx->str : ""));
-        }
-        if (!byte_level_ok(&seq->arr[3], false)) return fail(t, XLLM_ERR_UNSUPPORTED, kUnsupported);
-        t->hf_pattern = 3;
-        t->hf_digits = 3;
-      } else {
-      if (!seq || seq->type != JVal::kArr || seq->arr.size() != 2) return fail(t, XLLM_ERR_UNSUPPORTED, kUnsupported);
-      const JVal& sp = seq->arr[0];
-      const JVal* st = sp.get("type");
-      const JVal* pat = sp.get("pattern");
-      const JVal* rx = pat ? pat->get("Regex") : nullptr;
-      const JVal* beh = sp.get("behavior");
-      if (!st || st->type != JVal::kStr || st->str != "Split" || !rx || rx->type != JVal::kStr || !beh ||
-          beh->type != JVal::kStr || beh->str != "Isolated" || !flag_false_or_absent(&sp, "invert") ||
-          !byte_level_ok(&seq->arr[1], false))
-        return fail(t, XLLM_ERR_UNSUPPORTED, kUnsupported);
-      if (rx->str == kP3) t->hf_digits = 3;
-      else if (rx->str == kP1) t->hf_digits = 1;
-      else return fail(t, XLLM_ERR_UNSUPPORTED, std::string(kUnsupported) + "; got regex " + rx->str);
-      t->hf_pattern = 2;
-      }
-    } else {
-      return fail(t, XLLM_ERR_UNSUPPORTED, kUnsupported);
+    static const Layout kLayouts[] = {
+        {0, {}, 1, 3},                   // GPT-2: a bare ByteLevel
+        {1, {kP3}, 2, 3},                // cl100k family, Llama-3
+        {1, {kP1}, 2, 1},                // cl100k family, Qwen2
+        {3, {kDs1, kDs2, kDs3}, 3, 3},   // DeepSeek-V3 / R1
+    };
+    const JVal* ty = pre ? pre->get("type") : nullptr;
+    const JVal* seq = pre ? pre->get("pretokenizers") : nullptr;
+    const bool is_seq = ty && ty->type == JVal::kStr && ty->str == "Sequence" && seq && seq->type == JVal::kArr &&
+                        seq->arr.size() >= 2;
+    if (!is_seq && !(ty && ty->type == JVal::kStr && ty->str == "ByteLevel")) return fail(t, XLLM_ERR_UNSUPPORTED, kUnsupported);
+    const size_t n_splits = is_seq ? seq->arr.size() - 1 : 0;
+    if (!byte_level_ok(is_seq ? seq->arr.back() : *pre, !is_seq)) return fail(t, XLLM_ERR_UNSUPPORTED, kUnsupported);
+    std::vector<const std::string*> regex(n_splits);
+    for (size_t k = 0; k < n_splits; ++k)
+      if (!(regex[k] = split_regex(seq->arr[k]))) return fail(t, XLLM_ERR_UNSUPPORTED, kUnsupported);
+    const Layout* layout = nullptr;
+    size_t matched = 0;   // the most leading Split entries that a layout of this length accepts
+    for (const Layout& l : kLayouts) {
+      if (l.n_splits != n_splits) continue;
+      size_t k = 0;
+      while (k < n_splits && *regex[k] == l.splits[k]) ++k;
+      if (k == n_splits) layout = &l;
+      matched = std::max(matched, k);
     }
+    if (!layout) return fail(t, XLLM_ERR_UNSUPPORTED, std::string(kUnsupported) + "; got regex " + *regex[matched]);
+    t->hf_pattern = layout->pattern;
+    t->hf_digits = layout->digits;
   }
 
   // ---- vocabulary
