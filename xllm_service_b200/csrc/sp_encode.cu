@@ -1172,6 +1172,19 @@ struct ExpReq {
 };
 // per warp: symbol columns for the words the memo does not know yet, the window's text and its words' owner lanes
 constexpr int kExpWords = 64;        // words an express step resolves: lane k takes words k and k + 32
+// What express_run keeps of its request in shared memory rather than in registers across the steps: values read
+// once a step (the row) or only by the cold paths (long words, the end of the run)
+struct ExpRunRec {
+  int32_t* out;                      // the request's row
+  int32_t cap;                       // ids that fit the row
+  uint32_t vlen;                     // v of the end of the text
+  uint32_t nunits;                   // aligned 16-byte units that hold text
+  uint32_t A;                        // the text's first byte's offset from the aligned address below it
+  int32_t n_long;                    // long words this request sent through the cooperative path
+  int32_t unk_end;                   // the id count right after a word that ended in an unknown symbol, else -1:
+                                     // ExpReq::U is unk_end == n_out (every word the step emits has an id)
+};
+static_assert(sizeof(ExpRunRec) == 32, "the run record is budgeted at 32 B per warp (DESIGN 4.2)");
 template <bool SMALL>
 struct ExpSmemT {
   uint32_t S[kMaxSym * 32];
@@ -1179,7 +1192,10 @@ struct ExpSmemT {
   uint4 txt_front;                   // read (and masked off) by the key of a word at the window's first byte
   uint4 txt[kExpWin / 16 + 1];       // the window (16 bytes per lane) + 16 bytes a word's key read may touch past it
   uint8_t own[kExpWords];            // own[i]: the lane whose first start is word i (where some lane's is)
+  ExpRunRec run;
 };
+static_assert(sizeof(ExpSmemT<true>) == 4736 && sizeof(ExpSmemT<false>) == 6784,
+              "per-warp shared memory of the express kernel as budgeted in DESIGN 4.2");
 constexpr int kExpLongWords = 4;     // express_run: long words a request may put through the cooperative path ...
 constexpr int kExpLongEvery = 512;   // ... at a density above one per this many bytes before it is handed over
 // what the buffer-path kernel needs to take a request over where the express kernel stopped
@@ -1403,20 +1419,20 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
                                                 MemoRef memo, bool* failed) {
   // 32-bit coordinates: v = byte offset from the 16-byte-aligned address at or below the request's first byte
   const uint32_t A = (uint32_t)(reinterpret_cast<uintptr_t>(rs.src) & 15u);
-  const uint32_t* const base = reinterpret_cast<const uint32_t*>(rs.src - A);
   const uint4* const base16 = reinterpret_cast<const uint4*>(rs.src - A);
-  const uint32_t vlen = rs.len + A;                 // end of the text
-  const uint32_t nwords = (vlen + 3u) >> 2;         // aligned 4-byte words that hold text (express_long_word)
-  const uint32_t nunits = (vlen + 15u) >> 4;        // aligned 16-byte units that hold text
+  // the same values from every lane; the row's address is one 64-bit value there: an id's address is then one wide
+  // multiply-add from it (rebuilt from the kernel's ids parameter and a 64-bit row index, it takes four instructions)
+  {
+    const uint32_t vlen = rs.len + A;
+    sm.run = ExpRunRec{rs.out, rs.cap > 0x7fffffffll ? 0x7fffffff : (int32_t)rs.cap, vlen, (vlen + 15u) >> 4, A, 0,
+                       rs.U ? (int32_t)rs.n_out : -1};
+  }
+  int32_t* const& out = sm.run.out;
+  const int32_t& cap = sm.run.cap;
+  const uint32_t& vlen = sm.run.vlen;               // end of the text
+  const uint32_t& nunits = sm.run.nunits;
   bool P = rs.P;
   bool S = rs.S;
-  bool U = rs.U;
-  int n_long = 0;             // long words this request sent through the cooperative path
-  // the row's address held as one 64-bit value: an id's address is then one wide multiply-add from it (rebuilt from
-  // the kernel's ids parameter and a 64-bit row index, it takes four instructions per word)
-  int32_t* out = rs.out;
-  asm("" : "+l"(out));
-  const int32_t cap = rs.cap > 0x7fffffffll ? 0x7fffffff : (int32_t)rs.cap;
   int32_t n_out = (int32_t)rs.n_out;
   const uint32_t lt = (1u << lane) - 1u;
   auto load_window = [&](uint32_t at) {             // the 32 aligned 16-byte units from the one that holds byte `at`
@@ -1503,13 +1519,16 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
       // a text dense in long words (natural text: one in ~100 bytes) is better off in the buffer-path kernel, which
       // merges words of up to 32 symbols 32 at a time in lane columns: after kExpLongWords of them at more than one
       // per kExpLongEvery bytes the rest of the request is handed over
-      ++n_long;
-      const bool dense = n_long > kExpLongWords && (uint32_t)n_long * (uint32_t)kExpLongEvery > wb + s0 - A;
+      const int32_t n_long = sm.run.n_long + 1;
+      __syncwarp();
+      if (lane == 0) sm.run.n_long = n_long;
+      const bool dense = n_long > kExpLongWords && (uint32_t)n_long * (uint32_t)kExpLongEvery > wb + s0 - sm.run.A;
+      const bool U = sm.run.unk_end == n_out;
       ExpLongWord r{0u, n_out, false, U};
-      if (!dense) r = express_long_word<SMALL>(T, sm, base, nwords, vlen, wb + s0, P || (!S && s0 > skip), out, cap,
-                                              n_out, U, lane);
+      if (!dense) r = express_long_word<SMALL>(T, sm, reinterpret_cast<const uint32_t*>(base16), (vlen + 3u) >> 2, vlen,
+                                              wb + s0, P || (!S && s0 > skip), out, cap, n_out, U, lane);
       n_out = r.n_out;
-      U = r.unk;
+      sm.run.unk_end = r.unk ? r.n_out : -1;   // the same in every lane
       if (!r.done) {
         if (s0 > skip) {                           // hand over at the word, with the spaces in front of it consumed
           P = P || !S;
@@ -1698,7 +1717,6 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
       exp_store<SMALL>(row + oA, valA, cntA, fits, cap - n_out - oA);
       if (c0 | c1 | c2) exp_store<SMALL>(row + oB, valB, cntB, fits, cap - n_out - oB);
       n_out += totalA + totalB;
-      U = false;
 #ifdef XLLM_EXP_STATS
       { const unsigned long long t = clock64(); cyc_window += t_vote - t_step; cyc_probe += t_probe - t_vote; cyc_emit += t - t_probe; ++n_timed; }
 #endif
@@ -1728,23 +1746,40 @@ __device__ __forceinline__ uint32_t express_run(const SpDev& T, SM& sm, ExpReq& 
 #endif
   rs.P = P;
   rs.S = S;
-  rs.U = U;
+  rs.U = sm.run.unk_end == n_out;
   rs.n_out = n_out;
   __syncwarp();
-  return v - A;
+  return v - sm.run.A;
 }
 
 // The express kernel: every request starts here when the model allows it (split_mode 1, remove_extra_whitespaces,
 // normalised text).  A request it carries to the end is finished (a pending U+2581 is the trailing space the
 // normalizer strips); one it cannot is handed to the buffer-path kernel with its position, id count and
-// whitespace state, through legacy_list / resume.  kExpWarps independent warps per block.
-constexpr int kExpWarps = 4;
-// 6 blocks of 4 warps: 80 registers, 24 warps per SM (64 registers spill heavily in the 64-word step, 96 leave 20 warps)
+// whitespace state, through legacy_list / resume.  Independent warps, up to ExpShape<SMALL>::kWarps per block (fewer
+// for small batches: sp_encode_plan).
+// Block shape per instantiation.  Narrow ids (4 736 B per warp): 2 blocks of 14 warps, 72 registers, 28 warps per SM;
+// 2 x (66 304 + 1 024 reserved) = 134 656 B of shared memory stay inside the 132 KB (135 168 B) carve-out, so L1, which
+// serves the hot memo slots, keeps ~124 KB.  7 blocks of 4 warps would need the 164 KB carve-out (~92 KB of L1).  Wide
+// ids (6 784 B per warp): 6 blocks of 4 warps, 80 registers, 24 warps per SM, 196 KB carve-out.  64 registers spill
+// heavily in the 64-word step, 96 leave 20 warps.
+#ifndef XLLM_EXP_WARPS
+#define XLLM_EXP_WARPS 14
+#endif
 #ifndef XLLM_EXP_MIN_BLOCKS
-#define XLLM_EXP_MIN_BLOCKS 6
+#define XLLM_EXP_MIN_BLOCKS 2
 #endif
 template <bool SMALL>
-__global__ void __launch_bounds__(kExpWarps * 32, XLLM_EXP_MIN_BLOCKS) sp_express_kernel(
+struct ExpShape {
+  static constexpr int kWarps = SMALL ? XLLM_EXP_WARPS : 4;
+  static constexpr int kMinBlocks = SMALL ? XLLM_EXP_MIN_BLOCKS : 6;
+  static constexpr size_t kSmem = kWarps * sizeof(ExpSmemT<SMALL>);   // per block
+  static constexpr size_t kSmemPerSm = kMinBlocks * (kSmem + 1024);     // + the 1 KB sm_90 reserves per block
+};
+// the default narrow-id shape keeps the 132 KB carve-out (variant builds that set another shape may need more)
+static_assert(XLLM_EXP_WARPS != 14 || XLLM_EXP_MIN_BLOCKS != 2 || ExpShape<true>::kSmemPerSm <= 132 * 1024,
+              "the narrow-id express blocks no longer fit the 132 KB carve-out: L1 would shrink to ~92 KB");
+template <bool SMALL>
+__global__ void __launch_bounds__(ExpShape<SMALL>::kWarps * 32, ExpShape<SMALL>::kMinBlocks) sp_express_kernel(
     const uint8_t* __restrict__ text, const int64_t* __restrict__ offsets, int n_req, int32_t* __restrict__ ids,
     int64_t ids_stride, int32_t* __restrict__ n_ids, int32_t* __restrict__ status, const __grid_constant__ SpDev T,
     unsigned int* __restrict__ task_counter, int32_t* __restrict__ legacy_list, unsigned int* __restrict__ legacy_count,
@@ -1795,7 +1830,7 @@ __global__ void __launch_bounds__(kExpWarps * 32, XLLM_EXP_MIN_BLOCKS) sp_expres
   if (T.warp_ns && lane == 0) {
     unsigned long long t1;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-    T.warp_ns[blockIdx.x * kExpWarps + (threadIdx.x >> 5)] = t1 - warp_t0;
+    T.warp_ns[blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)] = t1 - warp_t0;
   }
 }
 
@@ -2776,6 +2811,32 @@ static size_t nfc_verdict_offset(int n) {
 // resident blocks of hf_nfc_verify_kernel per SM (its __launch_bounds__ minimum)
 constexpr int kNfcBlocksPerSm = 8;
 
+// Opts sp_express_kernel<SMALL> in to its blocks' shared memory on device d, asks for the smallest carve-out that
+// holds ExpShape's resident blocks (whatever shared memory does not take is L1, which serves the hot memo slots), and
+// returns the resident blocks per SM.  The carve-out is asked for as a percentage of the SM's shared-memory maximum,
+// which the driver rounds up to the next capacity the SM supports; the percentage is taken from that capacity,
+// rounded down, so that it rounds up to the capacity itself (sm_90's capacities are 8 KB or more apart, 1 % of
+// 228 KB is 2.3 KB).
+template <bool SMALL>
+static cudaError_t express_setup(int d, int* per_sm) {
+  using X = ExpShape<SMALL>;
+  static constexpr int kCapacityKb[] = {0, 8, 16, 32, 64, 100, 132, 164, 196, 228};   // sm_90
+  int max_smem = 0, reserved = 0;
+  cudaError_t e = cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerMultiprocessor, d);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, d);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(sp_express_kernel<SMALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)X::kSmem);
+  if (e != cudaSuccess) return e;
+  const size_t need = (size_t)X::kMinBlocks * (X::kSmem + (size_t)reserved);
+  size_t cap = (size_t)max_smem;
+  for (const int kb : kCapacityKb)
+    if ((size_t)kb * 1024 >= need) { cap = (size_t)kb * 1024; break; }
+  const int pct = max_smem > 0 && cap < (size_t)max_smem ? (int)(cap * 100 / (size_t)max_smem) : 100;
+  e = cudaFuncSetAttribute(sp_express_kernel<SMALL>, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(per_sm, sp_express_kernel<SMALL>, X::kWarps * 32, X::kSmem);
+  if (e == cudaSuccess && *per_sm < 1) *per_sm = 1;
+  return e;
+}
+
 cudaError_t sp_encode_plan(const SpDev& dev, int n_req, bool memo, bool warm, SpEncodePlan* plan, bool nfc_verify) {
   SpEncodePlan& p = *plan;
   p = SpEncodePlan();
@@ -2783,17 +2844,8 @@ cudaError_t sp_encode_plan(const SpDev& dev, int n_req, bool memo, bool warm, Sp
   int d = 0;   // get() sets it before the setup runs
   const int n_sm = g_sp_once.get(
       [&] {
-        for (int s = 0; s < 2; ++s) {
-          int& b = g_exp_per_sm[d][s];
-          const cudaError_t r =
-              s ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, sp_express_kernel<true>, kExpWarps * 32,
-                                                                kExpWarps * sizeof(ExpSmemT<true>))
-                : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, sp_express_kernel<false>, kExpWarps * 32,
-                                                                kExpWarps * sizeof(ExpSmemT<false>));
-          if (r != cudaSuccess) return r;
-          if (b < 1) b = 1;
-        }
-        return cudaSuccess;
+        const cudaError_t r = express_setup<false>(d, &g_exp_per_sm[d][0]);
+        return r != cudaSuccess ? r : express_setup<true>(d, &g_exp_per_sm[d][1]);
       },
       &e, &d);
   if (e != cudaSuccess) return e;
@@ -2816,9 +2868,17 @@ cudaError_t sp_encode_plan(const SpDev& dev, int n_req, bool memo, bool warm, Sp
       const int v = atoi(w);
       if (v > 0 && v < per_sm) per_sm = v;
     }
-    const int need = (n + kExpWarps - 1) / kExpWarps;
-    p.express_blocks = n_sm * per_sm < need ? n_sm * per_sm : need;
-    if (p.express_blocks * kExpWarps > p.warp_ns) p.warp_ns = p.express_blocks * kExpWarps;
+    // warps per block: the full shape once the batch fills every resident block; below that as few as spread the
+    // requests over all of them, but at least 4 (a small batch then runs as before the 14-warp blocks: on as many
+    // SMs as it has requests / 4, one warp per scheduler)
+    const int max_warps = small ? ExpShape<true>::kWarps : ExpShape<false>::kWarps;
+    const int slots = n_sm * per_sm;
+    int warps = (n + slots - 1) / slots;
+    warps = warps < 4 ? 4 : (warps > max_warps ? max_warps : warps);
+    const int need = (n + warps - 1) / warps;
+    p.express_warps = warps;
+    p.express_blocks = slots < need ? slots : need;
+    if (p.express_blocks * warps > p.warp_ns) p.warp_ns = p.express_blocks * warps;
   }
   // scratch: [deferred requests n][handed-over requests n, to 16 bytes][resume records n]
   p.scratch_bytes = (((size_t)n * 8 + 15) & ~(size_t)15) + (size_t)n * sizeof(ExpResume) + 16;
@@ -2889,7 +2949,7 @@ static cudaError_t launch_plan(const SpEncodePlan& p, EncodeArgs a) {
     int32_t* const legacy_list = static_cast<int32_t*>(a.scratch) + a.n_req;
     ExpResume* const resume =
         reinterpret_cast<ExpResume*>(static_cast<uint8_t*>(a.scratch) + (((size_t)a.n_req * 8 + 15) & ~(size_t)15));
-    sp_express_kernel<SMALL><<<p.express_blocks, kExpWarps * 32, kExpWarps * sizeof(ExpSmemT<SMALL>), a.stream>>>(
+    sp_express_kernel<SMALL><<<p.express_blocks, p.express_warps * 32, p.express_warps * sizeof(ExpSmemT<SMALL>), a.stream>>>(
         a.text, a.offsets, a.n_req, a.ids, a.ids_stride, a.n_ids, a.status, a.dev, a.counters + 3, legacy_list,
         a.counters + 4, resume, a.memo_table, a.memo_mask);
     const cudaError_t e = cudaGetLastError();

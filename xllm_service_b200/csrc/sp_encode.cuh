@@ -132,7 +132,8 @@ struct SpEncodePlan {
   bool express = false;    // the express kernel runs first (memo on, not warm, sp_express_model)
   bool long_pass = false;  // the long-word kernel runs last, over the deferred requests (BPE models)
   int kernels = 0;         // kernels enqueued
-  int express_blocks = 0;  // blocks of 4 warps
+  int express_blocks = 0;  // blocks of the express kernel ...
+  int express_warps = 0;   // ... of this many warps (at most its block shape, sp_encode.cu ExpShape)
   int grid = 0;            // warps (= blocks) of the buffer-path throughput kernel: as many as its shared memory lets
                            // the SMs hold, at most n_req
   int grid_long = 0;       // warps of the long-word kernel
