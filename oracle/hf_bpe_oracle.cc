@@ -6,7 +6,8 @@
 //   xllm_service/tokenizer/tokenizers/src/lib.rs:38-41,83-99   Tokenizer::encode(text, add_special_tokens)
 // The arithmetic is the Rust crate `tokenizers` 0.21 (Cargo.toml:11, absent from the reference checkout); this file
 // restates its published pipeline for the configuration GPT-2 style models use:
-//   added_vocabulary.rs   text is first split on the added (special) tokens, leftmost-longest
+//   added_vocabulary.rs   text is first split on the added tokens that are not `normalized`, leftmost-longest; the
+//                         `normalized` ones are then matched the same way inside the pieces between those
 //   pre_tokenizers/byte_level.rs   regex split
 //        's|'t|'re|'ve|'m|'ll|'d| ?\p{L}+| ?\p{N}+| ?[^\s\p{L}\p{N}]+|\s+(?!\S)|\s+   then bytes -> GPT-2 byte chars
 //   pre_tokenizers/split.rs + byte_level.rs(use_regex = false)   the newer layout (Llama-3, Qwen2, OLMo-2 ...):
@@ -46,7 +47,8 @@ int uni_sub(uint32_t cp) {
 struct Hf {
   int32_t byte_sym[256];                                   // byte -> id of its byte-level char
   std::unordered_map<uint64_t, std::pair<uint32_t, int32_t>> merges;  // (a << 32 | b) -> (rank, new id)
-  std::vector<std::pair<std::string, int32_t>> added;      // special tokens matched on the raw text
+  std::vector<std::pair<std::string, int32_t>> added;      // added tokens matched on the raw text
+  std::vector<bool> added_normalized;                      // normalized: matched in the second pass only
   int pattern = 1;                                         // 1: GPT-2 ByteLevel regex, 2: cl100k family, 3: DeepSeek-V3
   int digits = 3;                                          // pattern 2: \p{N}{1,digits}
   bool ignore_merges = false;
@@ -317,17 +319,46 @@ void bpe_word(const Hf& h, const uint8_t* bytes, size_t n, std::vector<int32_t>*
   for (int i = 0; i >= 0 && (size_t)i < n; i = s[i].next) ids->push_back(s[i].id);
 }
 
+// leftmost-longest added token of one pass (normalized == which) in text[from, to): its start (to = none)
+size_t next_added(const Hf& h, const uint8_t* text, size_t from, size_t to, bool which, size_t* len, int32_t* id) {
+  for (size_t p = from; p < to; ++p) {
+    size_t best = 0;
+    for (size_t a = 0; a < h.added.size(); ++a) {
+      const std::string& s = h.added[a].first;
+      if (h.added_normalized[a] == which && s.size() <= to - p && s.size() > best && memcmp(text + p, s.data(), s.size()) == 0) {
+        best = s.size();
+        *id = h.added[a].second;
+      }
+    }
+    if (best) { *len = best; return p; }
+  }
+  return to;
+}
+
 long encode(const Hf& h, const uint8_t* text, size_t len, std::vector<int32_t>* ids) {
+  // added_vocabulary.rs extract_and_normalize: split on the non-normalized tokens, then match the normalized ones
+  // inside the pieces between them only
+  std::vector<std::pair<size_t, size_t>> cut;   // (start, length) of every added token, in text order
+  std::vector<int32_t> cut_id;
+  for (size_t pos = 0; pos <= len;) {
+    size_t l1 = 0, l2 = 0;
+    int32_t id1 = -1, id2 = -1;
+    const size_t at1 = next_added(h, text, pos, len, false, &l1, &id1);
+    for (size_t q = pos; q < at1;) {
+      const size_t at2 = next_added(h, text, q, at1, true, &l2, &id2);
+      if (at2 == at1) break;
+      cut.emplace_back(at2, l2);
+      cut_id.push_back(id2);
+      q = at2 + l2;
+    }
+    if (at1 == len) break;
+    cut.emplace_back(at1, l1);
+    cut_id.push_back(id1);
+    pos = at1 + l1;
+  }
   size_t pos = 0;
-  while (pos <= len) {
-    // next added token at or after pos (leftmost, longest at that position)
-    size_t best_at = len, best_len = 0;
-    int32_t best_id = -1;
-    for (size_t p = pos; p < len && best_id < 0; ++p)
-      for (const auto& a : h.added)
-        if (a.first.size() <= len - p && a.first.size() > best_len && memcmp(text + p, a.first.data(), a.first.size()) == 0) {
-          best_at = p; best_len = a.first.size(); best_id = a.second;
-        }
+  for (size_t k = 0; k <= cut.size(); ++k) {
+    const size_t best_at = k < cut.size() ? cut[k].first : len;
     // ordinary text [pos, best_at)
     std::vector<Ch> c;
     for (size_t p = pos; p < best_at;) {
@@ -349,9 +380,9 @@ long encode(const Hf& h, const uint8_t* text, size_t len, std::vector<int32_t>* 
       }
       bpe_word(h, text + b, e - b, ids);
     }
-    if (best_id < 0) break;
-    ids->push_back(best_id);
-    pos = best_at + best_len;
+    if (k == cut.size()) break;
+    ids->push_back(cut_id[k]);
+    pos = best_at + cut[k].second;
   }
   return (long)ids->size();
 }
@@ -361,16 +392,18 @@ long encode(const Hf& h, const uint8_t* text, size_t len, std::vector<int32_t>* 
 extern "C" {
 
 // byte_sym[256]: id of each byte's byte-level char; merges: n x (left id, right id, new id), rank = index;
-// added: n_added strings (blob + offsets) with their ids.
+// added: n_added strings (blob + offsets) with their ids and `normalized` flags (null: none normalized).
 void* oracle_hf_new(const int32_t* byte_sym, const int32_t* merges, size_t n_merges, const char* added_blob,
-                    const int64_t* added_off, const int32_t* added_ids, size_t n_added) {
+                    const int64_t* added_off, const int32_t* added_ids, const uint8_t* added_normalized, size_t n_added) {
   Hf* h = new Hf();
   memcpy(h->byte_sym, byte_sym, sizeof(h->byte_sym));
   for (size_t i = 0; i < n_merges; ++i)
     h->merges.emplace(((uint64_t)(uint32_t)merges[3 * i] << 32) | (uint32_t)merges[3 * i + 1],
                       std::make_pair((uint32_t)i, merges[3 * i + 2]));
-  for (size_t i = 0; i < n_added; ++i)
+  for (size_t i = 0; i < n_added; ++i) {
     h->added.emplace_back(std::string(added_blob + added_off[i], (size_t)(added_off[i + 1] - added_off[i])), added_ids[i]);
+    h->added_normalized.push_back(added_normalized && added_normalized[i]);
+  }
   return h;
 }
 // pattern: 1 GPT-2 / 2 cl100k family (digits = K) / 3 DeepSeek-V3 three-stage split; vocab: raw bytes of every token (blob + offsets) with ids,

@@ -89,7 +89,7 @@ def lib():
         L.oracle_tik_vocab_size.restype = ctypes.c_long
         L.oracle_tik_encode.argtypes = [VP, ctypes.c_char_p, ctypes.c_size_t, VP, ctypes.c_size_t]
         L.oracle_tik_encode.restype = ctypes.c_long
-        L.oracle_hf_new.argtypes = [VP, VP, ctypes.c_size_t, ctypes.c_char_p, VP, VP, ctypes.c_size_t]
+        L.oracle_hf_new.argtypes = [VP, VP, ctypes.c_size_t, ctypes.c_char_p, VP, VP, VP, ctypes.c_size_t]
         L.oracle_hf_new.restype = VP
         L.oracle_hf_configure.argtypes = [VP, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_char_p, VP, VP,
                                           ctypes.c_size_t]
@@ -426,15 +426,31 @@ class HfBpeOracle:
             a, b = e if isinstance(e, list) else e.split(" ")
             mg.append((vocab[a], vocab[b], vocab[a + b]))
         merges = np.array(mg, dtype=np.int32).reshape(-1, 3)
-        added = [(t["content"].encode("utf-8"), t["id"]) for t in d.get("added_tokens", [])]
+        # the ids `tokenizers` gives added tokens when it loads the file (AddedVocabulary::add_tokens, in list
+        # order), whatever ids the file lists: a content that is a vocabulary entry or an earlier added token keeps
+        # that id, any other gets len(vocab), or one past the largest added id once that is at least len(vocab)
+        given, flags, listed = {}, {}, []
+        for t in d.get("added_tokens", []):
+            c = t["content"]
+            f = (bool(t.get("special", False)), bool(t.get("normalized", not t.get("special", False))))
+            assert flags.setdefault(c, f) == f, "added token %r listed twice with different flags" % c
+            if c not in given:
+                listed.append(t)
+                top = max(given.values(), default=None)
+                given[c] = vocab[c] if c in vocab else (len(vocab) if top is None or top < len(vocab) else top + 1)
+        self.added = [(t["content"], given[t["content"]], bool(t.get("special", False)),
+                       bool(t.get("normalized", not t.get("special", False)))) for t in listed]
+        added = [(c.encode("utf-8"), i) for c, i, _, _ in self.added]
         blob = b"".join(a for a, _ in added)
         off = np.zeros(len(added) + 1, dtype=np.int64)
         if added:
             np.cumsum([len(a) for a, _ in added], out=off[1:])
         ids = np.array([i for _, i in added], dtype=np.int32)
-        self._keep = (byte_sym, merges, blob, off, ids)
+        norm = np.array([n for _, _, _, n in self.added] or [0], dtype=np.uint8)
+        self._keep = (byte_sym, merges, blob, off, ids, norm)
         self._h = lib().oracle_hf_new(byte_sym.ctypes.data, merges.ctypes.data, merges.shape[0],
-                                      ctypes.c_char_p(blob), off.ctypes.data, ids.ctypes.data, len(added))
+                                      ctypes.c_char_p(blob), off.ctypes.data, ids.ctypes.data, norm.ctypes.data,
+                                      len(added))
         u2b = {c: b for b, c in b2u.items()}
         raw = [(bytes(u2b[ch] for ch in tok), i) for tok, i in vocab.items() if all(ch in u2b for ch in tok)]
         vblob = b"".join(r for r, _ in raw)
@@ -456,6 +472,35 @@ class HfBpeOracle:
                         (self.suffix_ids if seen else self.prefix_ids).extend(
                             pr["special_tokens"][it["SpecialToken"]["id"]]["ids"])
         self.vocab_size = max(vocab.values()) + 1
+        self._vocab_id = vocab.get
+        # Tokenizer::get_vocab_size(with_added_tokens = true): the vocabulary plus the added tokens it lacks
+        self.vocab_size_with_added = len(vocab) + len({i for _, i, _, _ in self.added if i >= len(vocab)})
+        self._token = {i: c for c, i in vocab.items()}
+        self._token.update({i: c for c, i, _, _ in self.added})
+        self._special = {i for _, i, s, _ in self.added if s}
+        self._u2b = {c: b for b, c in b2u.items()}
+
+    def token_to_id(self, content):
+        for c, i, _, _ in self.added:
+            if c == content:
+                return i
+        return self._vocab_id(content)
+
+    def decode(self, ids, skip_special_tokens=False):
+        """Tokenizer::decode: tokens (added ones too) through the ByteLevel decoder, each mapped back to bytes when all
+        its chars are in the byte alphabet and kept verbatim otherwise, the joined bytes read as String::from_utf8_lossy
+        does (Python's errors="replace" takes the same maximal subparts); unknown ids and, on request, special tokens
+        are left out."""
+        out = bytearray()
+        for i in ids:
+            t = self._token.get(int(i))
+            if t is None or (skip_special_tokens and int(i) in self._special):
+                continue
+            if all(ch in self._u2b for ch in t):
+                out += bytes(self._u2b[ch] for ch in t)
+            else:
+                out += t.encode("utf-8")
+        return bytes(out).decode("utf-8", errors="replace")
 
     def __del__(self):
         try:

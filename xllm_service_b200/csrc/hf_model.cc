@@ -10,7 +10,9 @@
 // normalizer null; pre_tokenizer one of the layouts in hf_load_model's kLayouts (GPT-2 ByteLevel, cl100k-family
 // Split, DeepSeek-V3's three Splits);
 // post_processor null, ByteLevel, or a TemplateProcessing whose `single` template only wraps the sequence in
-// special tokens; added tokens that are matched verbatim (normalized:false, no lstrip/rstrip/single_word).
+// special tokens; added tokens without lstrip/rstrip/single_word, matched verbatim: the normalized:false ones first,
+// the normalized:true ones between those (under normalizer NFC only NFC-inert normalized contents are taken, so
+// NFC(content) = content).
 // Tables: byte_mode (every byte is a symbol: the byte-level alphabet is a bijection byte <-> char), the pair
 // table comes straight from `merges` (priority = merge rank), split_mode 3 = the regex pre-tokenizer.
 #include <stdio.h>
@@ -181,6 +183,25 @@ std::string utf8_of(uint32_t cp) {
   return s;
 }
 
+// the bytes a token spelled in the byte-level alphabet stands for; false when a char is outside the alphabet
+bool byte_level_bytes(const std::string& tok, const std::unordered_map<uint32_t, uint8_t>& byte_of_cp, std::string* raw) {
+  const uint8_t* p = (const uint8_t*)tok.data();
+  const size_t n = tok.size();
+  size_t i = 0;
+  raw->clear();
+  while (i < n) {
+    uint32_t cp;
+    if (p[i] < 0x80) { cp = p[i]; i += 1; }
+    else if ((p[i] & 0xE0) == 0xC0 && i + 1 < n) { cp = ((p[i] & 0x1F) << 6) | (p[i + 1] & 0x3F); i += 2; }
+    else if ((p[i] & 0xF0) == 0xE0 && i + 2 < n) { cp = ((p[i] & 0x0F) << 12) | ((p[i + 1] & 0x3F) << 6) | (p[i + 2] & 0x3F); i += 3; }
+    else return false;
+    auto it = byte_of_cp.find(cp);
+    if (it == byte_of_cp.end()) return false;
+    raw->push_back((char)it->second);
+  }
+  return true;
+}
+
 int fail(SpTables* t, int code, const std::string& msg) {
   t->error = msg;
   return code;
@@ -349,28 +370,73 @@ int hf_load_model(const std::string& path_in, SpTables* t) {
     id_of.emplace(kv.first, id);
     max_id = id > max_id ? id : max_id;
   }
-  // ---- added tokens
+  // ---- added tokens, with the ids `tokenizers` gives them when it loads the file (AddedVocabulary::add_tokens, in
+  // list order) whatever ids the file lists: a content that is a model.vocab entry or an earlier added token keeps
+  // that id, any other gets len(model.vocab), or one past the largest added id once that is at least len(model.vocab)
+  struct Added {
+    std::string content;
+    int32_t id;
+    bool special, normalized;
+  };
+  std::vector<Added> added_list;
+  std::unordered_map<std::string, int32_t> added_id_of;
   const JVal* added = root.get("added_tokens");
   if (added && added->type == JVal::kArr) {
+    int32_t top = -1;
     for (const JVal& a : added->arr) {
       const JVal* content = a.get("content");
       const JVal* id = a.get("id");
       if (!content || content->type != JVal::kStr || content->str.empty() || !id || id->type != JVal::kNum)
         return fail(t, XLLM_ERR_FORMAT, "bad added_tokens entry");
-      // `normalized` only matters with a normalizer, and any normalizer was rejected above
       if (!flag_false_or_absent(&a, "single_word") || !flag_false_or_absent(&a, "lstrip") ||
           !flag_false_or_absent(&a, "rstrip"))
         return fail(t, XLLM_ERR_UNSUPPORTED, "added token '" + content->str + "': single_word/lstrip/rstrip are not supported on device");
       if (content->str.size() > 64) return fail(t, XLLM_ERR_UNSUPPORTED, "added token longer than 64 bytes");
-      t->added_tokens.emplace_back(content->str, (int32_t)id->num);
-      max_id = (int32_t)id->num > max_id ? (int32_t)id->num : max_id;
+      const bool special = !flag_false_or_absent(&a, "special");
+      const JVal* nz = a.get("normalized");
+      const bool normalized = nz && nz->type == JVal::kBool ? nz->b : !special;   // the library's default
+      if (added_id_of.count(content->str)) {
+        // an identical repeat is ignored, as the library does; one with other flags would make them depend on the
+        // library's bookkeeping (the special set keeps the first, the id's entry the last)
+        for (const auto& b : added_list)
+          if (b.content == content->str && (b.special != special || b.normalized != normalized))
+            return fail(t, XLLM_ERR_UNSUPPORTED, "added token '" + content->str + "' is listed twice with different flags");
+        continue;
+      }
+      // `normalized` tokens are matched in the second pass on the text itself: with normalizer NFC the device only
+      // encodes text NFC leaves unchanged, and the library matches NFC(content) there, so a content is taken only when
+      // every char of it is NFC-inert (then NFC(content) = content)
+      if (normalized && t->nfc_check) {
+        const uint8_t* u = (const uint8_t*)content->str.data();
+        for (size_t i = 0; i < content->str.size();) {
+          uint32_t cp = u[i];
+          int l = 1;
+          if (cp >= 0xF0) { cp &= 0x07; l = 4; } else if (cp >= 0xE0) { cp &= 0x0F; l = 3; } else if (cp >= 0xC0) { cp &= 0x1F; l = 2; }
+          for (int k = 1; k < l && i + k < content->str.size(); ++k) cp = (cp << 6) | (u[i + k] & 0x3F);
+          i += l;
+          if (cp >= 0x80 && cp < 0x110000 && (kUniStage2[(size_t)kUniStage1[cp >> 8] * 256 + (cp & 255)] & 4))
+            return fail(t, XLLM_ERR_UNSUPPORTED, "normalized added token '" + content->str + "' is not NFC-inert under normalizer NFC");
+        }
+      }
+      auto in_vocab = id_of.find(content->str);
+      const int32_t aid = in_vocab != id_of.end() ? in_vocab->second
+                          : (top < (int32_t)id_of.size() ? (int32_t)id_of.size() : top + 1);
+      top = std::max(top, aid);
+      added_id_of.emplace(content->str, aid);
+      added_list.push_back(Added{content->str, aid, special, normalized});
+      max_id = aid > max_id ? aid : max_id;
     }
     {   // the device keeps them in one blob addressed by 16-bit offsets (DeepSeek-V3: ~820 tokens, ~25 KB)
       size_t blob = 0;
-      for (const auto& a : t->added_tokens) blob += a.first.size();
-      if (t->added_tokens.size() > 2048 || blob > 65535)
+      for (const auto& a : added_list) blob += a.content.size();
+      if (added_list.size() > 2048 || blob > 65535)
         return fail(t, XLLM_ERR_UNSUPPORTED, "added tokens: more than 2048 of them or more than 65535 bytes in total");
     }
+    // the non-normalized tokens first: the device matches added_tokens[0, n_added_plain) in its first pass
+    for (int pass = 0; pass < 2; ++pass)
+      for (const auto& a : added_list)
+        if (a.normalized == (pass == 1)) t->added_tokens.emplace_back(a.content, a.id);
+    for (const auto& a : added_list) t->n_added_plain += !a.normalized;
   }
   const uint32_t V = (uint32_t)max_id + 1;
   t->byte_mode = true;
@@ -406,19 +472,7 @@ int hf_load_model(const std::string& path_in, SpTables* t) {
   t->piece_type.assign(V, 1);
   for (const auto& kv : id_of) {
     std::string raw;
-    const uint8_t* p = (const uint8_t*)kv.first.data();
-    size_t n = kv.first.size(), i = 0;
-    bool ok = true;
-    while (i < n) {
-      uint32_t cp;
-      if (p[i] < 0x80) { cp = p[i]; i += 1; }
-      else if ((p[i] & 0xE0) == 0xC0 && i + 1 < n) { cp = ((p[i] & 0x1F) << 6) | (p[i + 1] & 0x3F); i += 2; }
-      else if ((p[i] & 0xF0) == 0xE0 && i + 2 < n) { cp = ((p[i] & 0x0F) << 12) | ((p[i + 1] & 0x3F) << 6) | (p[i + 2] & 0x3F); i += 3; }
-      else { ok = false; break; }
-      auto it = byte_of_cp.find(cp);
-      if (it == byte_of_cp.end()) { ok = false; break; }
-      raw.push_back((char)it->second);
-    }
+    const bool ok = byte_level_bytes(kv.first, byte_of_cp, &raw);
     t->piece_str[(size_t)kv.second] = kv.first;
     t->piece_raw[(size_t)kv.second] = ok ? raw : kv.first;
     raw_ok[(size_t)kv.second] = ok;
@@ -434,12 +488,16 @@ int hf_load_model(const std::string& path_in, SpTables* t) {
     if (rc != XLLM_OK) return rc;
   }
   size_t n_extra = 0;
-  for (const auto& a : t->added_tokens) {
-    n_extra += id_of.find(a.first) == id_of.end();
-    t->piece_str[(size_t)a.second] = a.first;
-    t->piece_raw[(size_t)a.second] = a.first;
-    t->piece_type[(size_t)a.second] = 3;  // CONTROL-like: skipped by decode(skip_special_tokens)
-    if ((size_t)a.second < t->emit.size()) t->emit[(size_t)a.second] = a.second;
+  for (const auto& a : added_list) {
+    n_extra += id_of.find(a.content) == id_of.end();
+    t->piece_str[(size_t)a.id] = a.content;
+    // the ByteLevel decoder maps an added token like any other: to bytes when all its chars are in the byte
+    // alphabet, verbatim otherwise
+    std::string raw;
+    if (!byte_level_bytes(a.content, byte_of_cp, &raw)) raw = a.content;
+    t->piece_raw[(size_t)a.id] = raw;
+    t->piece_type[(size_t)a.id] = a.special ? 3 : 1;  // 3: skipped by decode(skip_special_tokens)
+    if ((size_t)a.id < t->emit.size()) t->emit[(size_t)a.id] = a.id;
   }
   t->vocab_size_override = (int32_t)(id_of.size() + n_extra);  // Tokenizer::get_vocab_size(with_added_tokens = true), lib.rs
   // ---- merges -> pair table (priority = index)

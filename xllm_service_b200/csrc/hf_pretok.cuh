@@ -2,7 +2,8 @@
 //
 // Device replacement for the two steps the Rust crate runs before BPE inside tokenizers_encode
 // (xllm_service/tokenizer/tokenizers/src/lib.rs:83-99 -> Tokenizer::encode):
-//   added_vocabulary.rs   split the text on the added (special) tokens, leftmost-longest, verbatim
+//   added_vocabulary.rs   split the text on the added tokens, leftmost-longest, verbatim: the normalized:false ones,
+//                         then the normalized:true ones between those
 //   pre_tokenizers/       split every remaining segment with the model's pattern, T.hf_pattern:
 //   1  GPT-2 ByteLevel (oracle/hf_bpe_oracle.cc gpt2_split)
 //        's|'t|'re|'ve|'m|'ll|'d| ?\p{L}+| ?\p{N}+| ?[^\s\p{L}\p{N}]+|\s+(?!\S)|\s+
@@ -18,7 +19,7 @@
 // along the buffer, done 32 bytes at a time with a warp-uniform carry.  So the warp decides all positions of the
 // staging buffer at once, in passes (hf_scan):
 //   A       hf_classify            class of every char (Unicode tables), UTF-8 validation, NFC quick check
-//   A2      hf_mark_added          added-token starts, leftmost-longest, non-overlapping
+//   A2      hf_mark_added          added-token starts, leftmost-longest, non-overlapping (one or two passes)
 //   B1      hf_mark_contractions   contraction starts (patterns 1, 2)
 //   C1, C2  hf_run_facts           swallowed CR/LFs, digit index in its run, CR/LF ahead in a whitespace run (2, 3)
 //   D1, D2  hf_ascii_runs          "punct + ASCII letters" tokens (3)
@@ -74,10 +75,11 @@ __device__ __forceinline__ uint8_t hf_class(const SpDev& T, uint32_t cp) {
   return __ldg(T.uni2 + (uint32_t)__ldg(T.uni1 + (cp >> 8)) * 256u + (cp & 255u));
 }
 
-// longest added token that is a prefix of p[0..avail); 0 = none.  *id = its token id.
-__device__ __forceinline__ int hf_added_len(const SpDev& T, const uint8_t* p, int avail, int32_t* id) {
+// longest added token of added[a0, a1) that is a prefix of p[0..avail); 0 = none.  *id = its token id.
+__device__ __forceinline__ int hf_added_len(const SpDev& T, const uint8_t* p, int avail, int32_t* id, uint32_t a0,
+                                            uint32_t a1) {
   int best = 0;
-  for (uint32_t a = 0; a < T.n_added; ++a) {
+  for (uint32_t a = a0; a < a1; ++a) {
     const int o = __ldg(T.added_off + a), l = (int)__ldg(T.added_off + a + 1) - o;
     if (l > avail || l <= best) continue;
     bool eq = true;
@@ -193,8 +195,10 @@ __device__ __forceinline__ int hf_classify(const SpDev& T, const uint8_t* nb, ui
   return __any_sync(kFull, bad) ? 1 : (__any_sync(kFull, nfc_bad) ? 2 : 0);
 }
 
-// ---- A2: added tokens, leftmost-longest, non-overlapping
-__device__ __forceinline__ void hf_mark_added(const SpDev& T, const uint8_t* nb, uint8_t* cls, int nlen, int lane) {
+// ---- A2: added tokens, leftmost-longest, non-overlapping, over added[0, n).  n = n_added, or in the two-pass kernels
+// n_added_plain: the normalized:false tokens, and hf_mark_added_second matches the normalized:true ones between them.
+__device__ __forceinline__ void hf_mark_added(const SpDev& T, const uint8_t* nb, uint8_t* cls, int nlen, uint32_t n,
+                                              int lane) {
   int cover = 0;
   for (int base = 0; base < nlen; base += 32) {
     const int p = base + lane;
@@ -203,7 +207,7 @@ __device__ __forceinline__ void hf_mark_added(const SpDev& T, const uint8_t* nb,
       const uint8_t b0 = nb[p];
       if ((T.added_first[b0 >> 5] >> (b0 & 31)) & 1u) {
         int32_t id;
-        al = hf_added_len(T, nb + p, nlen - p, &id);
+        al = hf_added_len(T, nb + p, nlen - p, &id, 0, n);
       }
     }
     uint32_t m = __ballot_sync(kFull, al > 0);
@@ -219,6 +223,43 @@ __device__ __forceinline__ void hf_mark_added(const SpDev& T, const uint8_t* nb,
     }
   }
   __syncwarp();
+}
+
+// The second pass: a normalized token matches only between the tokens of the first pass (avail ends at the next
+// one).  In a non-final buffer a first-pass token that the buffer end cuts off is not seen, so a match that reaches
+// the last added_max_len bytes is deferred: the returned bound (nlen when nothing is deferred) lies 9 bytes below its
+// start, the margin of the first pass, and the next buffer decides it.  Only the two-pass kernels (MODE 3) have it.
+__device__ __forceinline__ int hf_mark_added_second(const SpDev& T, const uint8_t* nb, uint8_t* cls, int nlen, bool final,
+                                                 int lane) {
+  int cover = 0, bound = nlen;
+  for (int base = 0; base < nlen; base += 32) {
+    const int p = base + lane;
+    int al = 0;
+    if (p < nlen && !hf_added(cls[p])) {
+      const uint8_t b0 = nb[p];
+      if ((T.added_first[b0 >> 5] >> (b0 & 31)) & 1u) {
+        int avail = nlen - p;
+        for (int k = 1; k < avail && k <= (int)T.added_max_len; ++k)
+          if (cls[p + k] & kHfAddedStart) { avail = k; break; }
+        int32_t id;
+        al = hf_added_len(T, nb + p, avail, &id, T.n_added_plain, T.n_added);
+      }
+    }
+    uint32_t m = __ballot_sync(kFull, al > 0);
+    while (m) {
+      const int bit = __ffs(m) - 1;
+      m &= m - 1;
+      const int q = base + bit;
+      const int l = __shfl_sync(kFull, al, bit);
+      if (q >= cover) {
+        for (int k = lane; k < l; k += 32) cls[q + k] = k == 0 ? kHfAddedStart : kHfInAdded;
+        cover = q + l;
+        if (!final && q + l > nlen - (int)T.added_max_len && q - 9 < bound) bound = q - 9;
+      }
+    }
+    __syncwarp();
+  }
+  return bound;
 }
 
 // ---- B1 (patterns 1, 2): an apostrophe starts a contraction token iff it is at a token start — i.e. the previous
@@ -453,8 +494,9 @@ __device__ __forceinline__ bool hf_token_start(int pattern, const uint8_t* nb, c
   return hf_rules1(nb, cls, nlen, p, q);
 }
 
-// nb[0..nlen) starts at a token start.  final: the text ends at nlen.
-template <typename SM>
+// nb[0..nlen) starts at a token start.  final: the text ends at nlen.  TWO: the model's added tokens are matched in
+// two passes (normalized:false, then normalized:true between those).
+template <bool TWO, typename SM>
 __device__ HfScan hf_scan(const SpDev& T, SM& sm, int nlen, bool final, int lane) {
   const uint8_t* nb = sm.nbuf;
   uint8_t* cls = reinterpret_cast<uint8_t*>(sm.S);
@@ -468,10 +510,17 @@ __device__ HfScan hf_scan(const SpDev& T, SM& sm, int nlen, bool final, int lane
   // HF kernels registers
   r.bad = hf_classify(T, nb, cls, aux, nlen, final, T.hf_pattern, lane);
   if (r.bad) return r;
-  if (T.n_added) hf_mark_added(T, nb, cls, nlen, lane);
+  int bound = nlen;
+  if constexpr (TWO) {
+    hf_mark_added(T, nb, cls, nlen, T.n_added_plain, lane);
+    bound = hf_mark_added_second(T, nb, cls, nlen, final, lane);
+  } else if (T.n_added) {
+    hf_mark_added(T, nb, cls, nlen, T.n_added, lane);
+  }
   if (T.hf_pattern != 3) hf_mark_contractions(nb, cls, nlen, T.hf_pattern == 2, lane);
   // non-final: a token is complete only if everything that decides its end is in the buffer
   int limit = final ? nlen : nlen - (int)T.added_max_len - 8;
+  if constexpr (TWO) limit = min(limit, bound);
   if (T.hf_pattern == 2 || T.hf_pattern == 3) hf_run_facts(cls, aux, nlen, T.hf_digits, final, T.hf_pattern == 3, lane, &limit);
   if (T.hf_pattern == 3) hf_ascii_runs(nb, cls, aux, nlen, lane);
   // ---- B2: token starts, compacted into wstart[]

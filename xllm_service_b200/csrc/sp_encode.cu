@@ -1860,14 +1860,15 @@ __device__ __forceinline__ int gather_chars(const SpDev& T, SM& sm, int ws, int 
 // Tokenises the complete words held in nbuf (all words when final) and keeps the incomplete tail.
 // HF: word boundaries come from the regex pre-tokenizer (hf_pretok.cuh); returns true when the word list
 // filled up and the kept tail has to be scanned again.
-// MODE: 0 SentencePiece BPE / tiktoken, 1 HF byte-level BPE (regex pre-tokenizer), 2 SentencePiece Unigram
+// MODE: 0 SentencePiece BPE / tiktoken, 1 HF byte-level BPE (regex pre-tokenizer), 2 SentencePiece Unigram,
+// 3 HF byte-level BPE whose added tokens need two matching passes (normalized:false and normalized:true ones)
 // WARM: with the warm-up pre-passes (1b below) for natural text.  A template parameter because carrying their state
 // through the in-order rounds slows the plain kernel on the headline workload: the launcher picks the WARM kernels
 // only when asked to (XLLM_SP_WARM=1).
 template <bool SMALL, bool LONG, int MODE, bool MEMO, bool WARM, typename SM>
 __device__ bool drain_pass(const SpDev& T, SM& sm, ReqState& rs, bool final, int lane, MemoRef memo) {
   static_assert(!WARM || (MEMO && !LONG && MODE != 2), "the warm-up pre-passes need the memo and the lane path");
-  constexpr bool HF = MODE == 1;
+  constexpr bool HF = MODE == 1 || MODE == 3;
   constexpr bool UNI = MODE == 2;
   const uint8_t* nb = sm.nbuf;
   int nlen = rs.nlen;
@@ -1883,7 +1884,7 @@ __device__ bool drain_pass(const SpDev& T, SM& sm, ReqState& rs, bool final, int
   int hf_tail = 0;
   bool hf_capped = false;
   if constexpr (HF) {
-    const HfScan sc = hf_scan(T, sm, nlen, final, lane);
+    const HfScan sc = hf_scan<MODE == 3>(T, sm, nlen, final, lane);
     if (sc.bad) { rs.bad_input = (int8_t)sc.bad; return false; }
     nwords = sc.nwords;
     hf_tail = sc.tail_start;
@@ -2184,7 +2185,7 @@ __device__ bool drain_pass(const SpDev& T, SM& sm, ReqState& rs, bool final, int
     } else if (memo_hit) {
     } else if (HF && active && special) {
       int32_t id = 0;
-      hf_added_len(T, nb + ws, we - ws, &id);
+      hf_added_len(T, nb + ws, we - ws, &id, 0, T.n_added);
       sm.S[lane] = kResolvedFlag | (uint32_t)id;
       alive = 1u;
       cnt = 1;
@@ -2397,8 +2398,8 @@ __device__ bool drain_pass(const SpDev& T, SM& sm, ReqState& rs, bool final, int
 
 template <bool SMALL, bool LONG, int MODE, bool MEMO, bool WARM, typename SM>
 __device__ __forceinline__ void drain(const SpDev& T, SM& sm, ReqState& rs, bool final, int lane, MemoRef memo) {
-  if constexpr (MODE == 1) {
-    while (drain_pass<SMALL, LONG, 1, MEMO, WARM>(T, sm, rs, final, lane, memo)) {}
+  if constexpr (MODE == 1 || MODE == 3) {
+    while (drain_pass<SMALL, LONG, MODE, MEMO, WARM>(T, sm, rs, final, lane, memo)) {}
   } else {
     drain_pass<SMALL, LONG, MODE, MEMO, WARM>(T, sm, rs, final, lane, memo);
   }
@@ -2415,7 +2416,7 @@ __global__ void __launch_bounds__(32, LONG ? 8 : ((MODE != 2 && !WARM) ? 16 : 27
     int64_t ids_stride, int32_t* __restrict__ n_ids, int32_t* __restrict__ status, const __grid_constant__ SpDev T,
     unsigned int* __restrict__ task_counter, int32_t* __restrict__ defer_list,
     unsigned int* __restrict__ defer_count, uint8_t* memo_table, uint32_t memo_mask) {
-  constexpr bool HF = MODE == 1;
+  constexpr bool HF = MODE == 1 || MODE == 3;
   const MemoRef memo{memo_table, memo_mask};
   extern __shared__ __align__(16) unsigned char smem_raw[];
   using SM = typename std::conditional<MODE == 2, WarpSmemUniT<SMALL>, WarpSmemT<SMALL, (MODE != 2 && !WARM) ? kHfRows : kMaxSym>>::type;
@@ -2480,13 +2481,13 @@ __global__ void __launch_bounds__(32, LONG ? 8 : ((MODE != 2 && !WARM) ? 16 : 27
       for (uint32_t pos = 0; pos < rs.len && !rs.bad_input; pos += kFastWin) {
         normalize_fast(T, sm, rs, pos, lane);  // byte mode: a verbatim copy
         if (rs.nlen > drain_at) {
-          drain<SMALL, LONG, 1, MEMO, WARM>(T, sm, rs, false, lane, memo);
+          drain<SMALL, LONG, MODE, MEMO, WARM>(T, sm, rs, false, lane, memo);
           // what is left is one unfinished pre-token (plus the look-ahead margin)
           if (rs.nlen > kLongEnterAt) rs.too_long = true;
           if (rs.too_long || rs.deferred || rs.bad_input) break;
         }
       }
-      if (!rs.too_long && !rs.deferred && !rs.bad_input) drain<SMALL, LONG, 1, MEMO, WARM>(T, sm, rs, true, lane, memo);
+      if (!rs.too_long && !rs.deferred && !rs.bad_input) drain<SMALL, LONG, MODE, MEMO, WARM>(T, sm, rs, true, lane, memo);
       if (!rs.too_long && !rs.deferred && !rs.bad_input) {
         if (lane < T.n_suffix) put_id(rs, rs.n_out + lane, T.suffix_ids[lane]);
         rs.n_out += T.n_suffix;
@@ -2628,7 +2629,7 @@ SpDeviceModel::~SpDeviceModel() {
 }
 
 int SpDeviceModel::upload(const SpTables& t) {
-  if (t.split_mode == 3 && (!t.byte_mode || t.added_tokens.size() > 256 || t.uni_stage1.empty())) {
+  if (t.split_mode == 3 && (!t.byte_mode || t.added_tokens.size() > 2048 || t.uni_stage1.empty())) {
     set_last_error("split_mode 3 (regex pre-tokenizer) needs byte-mode tables and the Unicode class tables");
     return XLLM_ERR_UNSUPPORTED;
   }
@@ -2682,6 +2683,8 @@ int SpDeviceModel::upload(const SpTables& t) {
       if (a.first.size() > dev_.added_max_len) dev_.added_max_len = (uint32_t)a.first.size();
     }
     dev_.n_added = (uint32_t)aid.size();
+    // the two-pass kernels are chosen only when the model has both kinds of added tokens
+    dev_.n_added_plain = t.n_added_plain != 0 && t.n_added_plain != aid.size() ? t.n_added_plain : 0;
     UP(blob, added_blob);
     UP(off, added_off);
     UP(aid, added_id);
@@ -2960,7 +2963,8 @@ static cudaError_t launch_plan(const SpEncodePlan& p, EncodeArgs a) {
   }
   // Unigram: Viterbi per word from a running score, so no word memo (the result depends on the prefix)
   if (a.dev.unigram) return launch_encode<SMALL, false, 2, false, false>(p.grid, a);
-  return a.dev.split_mode == 3 ? launch_bpe<SMALL, 1>(p, a) : launch_bpe<SMALL, 0>(p, a);
+  if (a.dev.split_mode != 3) return launch_bpe<SMALL, 0>(p, a);
+  return a.dev.n_added_plain != 0 ? launch_bpe<SMALL, 3>(p, a) : launch_bpe<SMALL, 1>(p, a);
 }
 
 cudaError_t sp_encode_launch(const SpDev& dev, const uint8_t* text, const int64_t* offsets, int n_req, int32_t* ids,

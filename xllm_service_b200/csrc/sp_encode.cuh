@@ -45,6 +45,7 @@ struct SpDev {
   const uint16_t* added_off;  // [n_added + 1]
   const int32_t* added_id;
   uint32_t n_added, added_max_len;
+  uint32_t n_added_plain;     // != 0: added[0, n_added_plain) are matched first, the rest only between them (MODE 3)
   uint32_t added_first[8];    // bit b set <=> some added token starts with byte b
   int32_t prefix_ids[4], suffix_ids[4];
   uint8_t n_prefix, n_suffix;

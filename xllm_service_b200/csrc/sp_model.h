@@ -60,8 +60,10 @@ struct SpTables {
   bool byte_mode = false;
   int32_t vocab_size_override = -1;
   // HF byte-level BPE (hf_model.cc): split_mode 3 = the GPT-2 regex pre-tokenizer over the raw bytes;
-  // added (special) tokens are matched verbatim in the text; template ids wrap every sequence
+  // added tokens are matched verbatim in the text, the first n_added_plain (normalized: false) in a first pass, the
+  // rest (normalized: true) in a second pass between those; template ids wrap every sequence
   std::vector<std::pair<std::string, int32_t>> added_tokens;
+  uint32_t n_added_plain = 0;
   std::vector<int32_t> prefix_ids, suffix_ids;
   int hf_pattern = 1;   // 1: ByteLevel's own GPT-2 regex, 2: Split(cl100k-family regex) + ByteLevel(use_regex = false)
   int hf_digits = 3;    // pattern 2: \p{N}{1,hf_digits}

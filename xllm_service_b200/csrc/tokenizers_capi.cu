@@ -22,6 +22,30 @@ struct LegacyTokenizer {
   std::string tmp_model_path;
 };
 
+// String::from_utf8_lossy: every maximal subpart of an ill-formed sequence becomes one U+FFFD
+std::string utf8_lossy(const std::string& in) {
+  const uint8_t* p = (const uint8_t*)in.data();
+  const size_t n = in.size();
+  std::string out;
+  out.reserve(n);
+  size_t i = 0;
+  while (i < n) {
+    const uint8_t b = p[i];
+    int len = 0;
+    uint8_t lo = 0x80, hi = 0xBF;   // range of the second byte
+    if (b < 0x80) len = 1;
+    else if (b >= 0xC2 && b <= 0xDF) len = 2;
+    else if (b >= 0xE0 && b <= 0xEF) { len = 3; lo = b == 0xE0 ? 0xA0 : 0x80; hi = b == 0xED ? 0x9F : 0xBF; }
+    else if (b >= 0xF0 && b <= 0xF4) { len = 4; lo = b == 0xF0 ? 0x90 : 0x80; hi = b == 0xF4 ? 0x8F : 0xBF; }
+    size_t k = 1;
+    while (len > 1 && (int)k < len && i + k < n && p[i + k] >= (k == 1 ? lo : 0x80) && p[i + k] <= (k == 1 ? hi : 0xBF)) ++k;
+    if (len > 0 && (int)k == len) out.append(in, i, (size_t)len);
+    else out += "\xEF\xBF\xBD";
+    i += len > 0 ? k : 1;
+  }
+  return out;
+}
+
 // SentencePieceProcessor::Decode for BPE pieces: U+2581 -> ' ', byte pieces -> raw bytes, control pieces
 // dropped, unknown -> " \xE2\x81\x87 " (the default unk_surface), leading space of the dummy prefix removed.
 std::string decode_ids(const xllm::SpTables& t, const uint32_t* ids, size_t n, bool skip_special) {
@@ -32,7 +56,8 @@ std::string decode_ids(const xllm::SpTables& t, const uint32_t* ids, size_t n, b
     const std::string& p = t.piece_str[ids[i]];
     if (t.byte_mode) {
       // tiktoken: tokens are raw byte strings (tiktoken_tokenizer.cpp:296-316); HF byte-level: the ByteLevel
-      // decoder maps the vocab spelling back to bytes, special tokens dropped on request (lib.rs:101-113)
+      // decoder maps the vocab spelling back to bytes, special tokens dropped on request (lib.rs:101-113), and the
+      // joined bytes read as String::from_utf8_lossy does
       if (!t.piece_raw.empty()) {
         if (!(skip_special && t.piece_type[ids[i]] == 3)) out += t.piece_raw[ids[i]];
       } else {
@@ -64,7 +89,7 @@ std::string decode_ids(const xllm::SpTables& t, const uint32_t* ids, size_t n, b
     }
     first = false;
   }
-  return out;
+  return t.byte_mode && !t.piece_raw.empty() ? utf8_lossy(out) : out;
 }
 
 LegacyTokenizer* make(const char* path) {
